@@ -8,7 +8,7 @@
 A "step" is one pass of the hot path over one batch of `--batch` decoded 1080p surfaces (NV12,
 NVDEC layout, pitch 2048): surfaces -> RGB -> {Histogram 3x16 int32, Resize 224x224 RGB24}.
   value   frames/s over all ranks with the surfaces already resident in HBM (CUDA events, max
-          over ranks); inputs rotate between two batches, each larger than the 126 MB L2.
+          over ranks); inputs rotate between two batches, each larger than the 50 MB L2.
   e2e     same metric end to end through the public pipeline API as configs[1] states it, on a stream with a real
           encoder's structure (scanner_b200/synth_h264.py; `e2e_ipcm_stream` repeats it on r01's lossless stream): the clips are
           TABLES of a database directory shared by all ranks (ingested H.264 + stored index); every step
@@ -18,8 +18,7 @@ NVDEC layout, pitch 2048): surfaces -> RGB -> {Histogram 3x16 int32, Resize 224x
           max over ranks), the steps summed; h2d/d2h bytes are the encoded bytes fed and the rows returned.
   roofline  the one kernel of the value leg (nv12_stream_kernel: histogram + resize in one pass over the
           surfaces): algorithmic bytes / its CUDA-event duration (scn_prof_*), against MEASURED_PEAKS.json's
-          HBM copy bandwidth.  The kernel is bound by instruction issue, not by HBM (profiles/r02_*): the
-          line says so and carries the issue-side evidence beside the HBM fraction.
+          HBM copy bandwidth when that file exists, else the H100 SXM data-sheet figure (3.35 TB/s).
   cpu_baseline  the reference's CPU path restated with the libraries it calls (FFmpeg H.264
           decode through cv2.VideoCapture, cv2.calcHist x3, cv2.resize; one clip per process, as
           the reference runs one pipeline instance per core) on a bounded sample of the same
@@ -29,7 +28,10 @@ configs[0] (Histogram on one 640x480 H.264 clip, CPU pipeline_instances=1, no GP
 as `config0_cpu`: the engine's CPU instance decodes with FFmpeg (libavcodec + libswscale through dlopen,
 scanner_b200/csrc/engine/swdec.h -- what the reference's SoftwareVideoDecoder is) and the stdlib Histogram runs on
 the CPU; a second or two, sampled rows checked against cv2 + the oracle.  Not part of `value` / `e2e`.
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR writes what the value leg's last timed step computed (rank 0) as
+float32 .npy files: hist.npy (batch, 3, 16) and resize_sample.npy, the Resize(224) rows of a fixed seeded sample of
+at most 64 of its frames, with their indices in resize_sample_frames.npy.  Inputs are seeded: the same arguments give
+the same inputs on every run.
 """
 import argparse
 import json
@@ -98,20 +100,14 @@ def config0_cpu(frames=720):
             "rows_checked_against_cv2_and_oracle": checked}
 
 
-# DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of the committed ncu --set full
-# capture of the bench's own launch shape (64 surfaces 1920x1080, pitch 2048, histogram + resize):
-# a CONSTANT from that profile, not a measurement of this run
-NCU_TRAFFIC = {"nv12_stream_kernel": {"bytes": None, "source": None}}
-_prof = os.path.join(ROOT, "profiles", "r02_nv12_stream_traffic.json")
-if os.path.exists(_prof):
-    NCU_TRAFFIC["nv12_stream_kernel"] = json.load(open(_prof))
+H100_HBM_GBS = 3350.0   # NVIDIA H100 SXM data sheet, HBM3
 
 
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
-        return json.load(open(p)).get("hbm_gbs", 6650.0), "measured"
-    return 6650.0, "fallback"
+        return json.load(open(p)).get("hbm_gbs", H100_HBM_GBS), "measured (burst copy, MEASURED_PEAKS.json)"
+    return H100_HBM_GBS, "H100 SXM data sheet"
 
 
 class ClockSampler(threading.Thread):
@@ -176,7 +172,7 @@ class ClockSampler(threading.Thread):
 
 def usable_cores():
     """Host cores this process may actually use: scheduler affinity capped by the cgroup CPU quota
-    (the GPU boxes report 128 logical CPUs but run the container under cpu.max = 16 cores)."""
+    (a container can see every host CPU and still run under a cgroup quota of a few cores)."""
     n = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
     try:
         quota, period = open("/sys/fs/cgroup/cpu.max").read().split()[:2]
@@ -299,7 +295,7 @@ def workload_config(args, batch):
     return {"workload": "configs[1]: 1080p H.264 decode + Resize(224x224) + Histogram",
             "frame": [H, W], "pitch": PITCH, "resize": [DH, DW], "frames_per_step": batch,
             "value_leg": "decoded NV12 surfaces resident in HBM -> streaming Histogram kernel + Resize kernel "
-                         "(two rotating input batches, each > the 126 MB L2)",
+                         "(two rotating input batches, each > the 50 MB L2)",
             "e2e_leg": "clips are tables of one database directory shared by all ranks (H.264: Intra16x16 + CAVLC key picture "
                        "every 30, motion-compensated P pictures, ~6 KB/frame; e2e_ipcm_stream: I_PCM IDR + P_Skip, ~105 KB/frame) "
                        "-> NVDEC -> GPU ops -> save stage into output tables, through scn_engine_run",
@@ -376,8 +372,8 @@ def default_instances(args, local_rank, world):
     from scanner_b200 import engine as E
     if args.instances > 0:
         return args.instances
-    # one decode session per NVDEC engine (7 on a B200) is the measured optimum (profiles/r01_e2e_engine_scaling.md),
-    # but never more threads than the rank's share of the host cores can keep fed
+    # one decode session per NVDEC engine (7 on an H100), but never more threads than the rank's share of the host
+    # cores can keep fed
     engines = E.nvdec_caps(local_rank).get("engines", 7) or 7
     return max(2, min(engines, 2 * usable_cores() // world))
 
@@ -546,9 +542,23 @@ def e2e_config1(args, R, sampler, stream_kind="pcm", steps=None):
                           "session_pictures_per_s_last_step": p["session_pictures_per_s"][-1],
                           "session_rate_spread_worst_step": max((max(r) - min(r)) / max(1, max(r)) for r in p["session_pictures_per_s"] if r),
                           "nvml_last_step": p["nvml"][-1], "numa_pinned_cpus": p["numa_pinned_cpus"]} for p in per_rank],
-            "bound": "NVDEC (7 engines/GPU; ~2 K pictures/s per session on the CAVLC stream, ~1.3 K on I_PCM); the pixel kernels "
-                     "take ~5 % of a step. All sessions of a rank run at the same rate within a step; slow steps are slow for "
-                     "every session (profiles/r02_e2e_variance.md)"}
+            "decoder": ("FFmpeg on the host (the GPU exposes no NVDEC engine to this process)"
+                        if stats.get("gpu_software_decode_sessions") else "NVDEC"),
+            "bound": "decode: session_pictures_per_s is the decode rate of every pipeline instance"}
+
+
+def dump_outputs(out_dir, hist, res):
+    """The last step's outputs as float32 .npy: every histogram, and the Resize rows of a fixed seeded sample of at
+    most 64 frames (all of them would be 4x the batch's uint8 bytes)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    n = hist.shape[0]
+    pick = np.sort(np.random.default_rng(0).choice(n, min(n, 64), replace=False))
+    sample = res.index_select(0, torch.from_numpy(pick).to(res.device))
+    np.save(os.path.join(out_dir, "hist.npy"), hist.cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "resize_sample.npy"), sample.cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "resize_sample_frames.npy"), pick.astype(np.float32))
 
 
 def _mmm(v):
@@ -585,7 +595,7 @@ def run_config1(args, R):
     R.barrier()
     e0.record()
     for i in range(args.steps):
-        step(i)
+        last = step(i)
     e1.record()
     sampler.sample_now()  # the steps are still executing: a sample under load even for short runs
     R.barrier()
@@ -594,6 +604,8 @@ def run_config1(args, R):
     clocks = sampler.result()
     sampler.stop_flag = True
     sampler.join(timeout=2)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last)
 
     # --- roofline leg: the same kernels on the same batches with per-kernel events (scn_prof_*), not used for
     # `value`.  In the value leg the Resize kernel runs on a forked stream next to the Histogram kernel; here each
@@ -612,7 +624,7 @@ def run_config1(args, R):
     # headline: a stream with a real encoder's structure and bitrate (CAVLC intra + motion-compensated pictures);
     # the lossless I_PCM / P_Skip stream r01 reported (105 KB per frame, nothing an encoder would produce) beside it
     e2e = e2e_config1(args, R, ClockSampler(local_rank), stream_kind="cavlc")
-    e2e_ipcm = e2e_config1(args, R, ClockSampler(local_rank), stream_kind="pcm", steps=max(2, min(args.steps, 5)))
+    e2e_ipcm = e2e_config1(args, R, ClockSampler(local_rank), stream_kind="pcm", steps=min(args.steps, 5))
     ms = R.max([ms])[0]
 
     if rank == 0:
@@ -629,19 +641,11 @@ def run_config1(args, R):
             separate_resize = True  # (SCN_NV12_RESIZE=fused would produce the Resize rows inside the streaming pass)
             alg = (B_ALG_HIST_NV12 if separate_resize else B_ALG_FUSED) * per_launch
             ach = alg / per_launch_s / 1e9
-            tr = NCU_TRAFFIC.get(kname, {})
-            roof = {"bound": "issue", "kernel": kname, "achieved": ach, "peak": peak, "unit": "GB/s",
-                    "frac": ach / peak, "peak_kind": peak_kind + " (burst copy, MEASURED_PEAKS.json)",
+            roof = {"kernel": kname, "achieved": ach, "peak": peak, "unit": "GB/s",
+                    "frac": ach / peak, "peak_kind": peak_kind,
                     "alg_bytes_per_launch": alg, "ms_per_launch": per_launch_s * 1e3,
-                    "traffic": tr.get("bytes") if B % 64 == 0 else None,
-                    "traffic_source": tr.get("source"),
-                    "bound_evidence": "instruction issue, not HBM: ~720 warp instructions per 1024 pixels with the ALU pipe "
-                                      "(carry-save histogram), the FMA pipe (exact colour matrix) and the issue port all "
-                                      "~70 % busy; measured pipe model in profiles/r02_pipe_ubench.md, ncu in "
-                                      "profiles/r02_nv12_stream.md, budget argument in DESIGN.md section 4",
-                    "launch_mode": ("Histogram by the streaming kernel, Resize by nv12_resize_kernel on a forked stream next to it "
-                                    "(measured faster than producing the Resize rows inside the streaming pass: "
-                                    "profiles/r02_nv12_stream.md)") if separate_resize else
+                    "launch_mode": "Histogram by the streaming kernel, Resize by nv12_resize_kernel on a forked stream next to it"
+                                   if separate_resize else
                                    "one kernel per 64 surfaces does Histogram and Resize in one pass",
                     "kernel_share_of_step": prof[kname]["ms"] / sum(v["ms"] for v in prof.values()),
                     "note": "kernels timed one at a time; in the value leg they overlap (ms_per_step / launches < their sum)",
@@ -940,9 +944,13 @@ def main():
     ap.add_argument("--e2e-frames", type=int, default=120, help="frames per clip in the e2e leg; configs[1] as stated: 300")
     ap.add_argument("--flow-clips", type=int, default=8, help="--config 3: clips; configs[3] as stated: 16")
     ap.add_argument("--flow-frames", type=int, default=96, help="--config 3: frames per clip; configs[3] as stated: 1200")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="--config 1: write the value leg's last-step outputs to DIR/<name>.npy (float32)")
     ap.add_argument("--instances", type=int, default=0,
                     help="pipeline instances per GPU for the e2e leg (0 = one per NVDEC engine, capped by the host cores)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.config != 1 or args.impl != "ours"):
+        ap.error("--dump-outputs is implemented for --config 1 of this implementation")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

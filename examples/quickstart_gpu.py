@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""The headline path on a B200: H.264 -> NVDEC -> Histogram + Resize(224) on the GPU -> stored tables.
+"""The headline path on an H100: H.264 -> NVDEC -> Histogram + Resize(224) on the GPU -> stored tables.
 
     python examples/quickstart_gpu.py [video.mp4]
 

@@ -7,7 +7,7 @@
 //   REGISTER_KERNEL(...).device().num_devices().batch().input_device().output_device().
 // Calling contract (SURVEY 8b): one evaluate thread owns a kernel instance; inputs are borrowed;
 // outputs are allocated by the kernel on its declared output device, exactly one per input row.
-// B200 addition: GPU kernels enqueue on device_stream(device) and need not synchronise.
+// Addition to the reference's API: GPU kernels enqueue on device_stream(device) and need not synchronise.
 #pragma once
 #include <functional>
 #include <map>
@@ -170,7 +170,7 @@ struct KernelDeclaration {
   i32 batch_size = 1;             // preferred rows per execute() when the graph does not say
   // columns that live on another device type than the kernel (e.g. encoded bytes for a GPU decoder)
   std::map<std::string, DeviceType> input_devices, output_devices;
-  // frame columns the kernel also accepts in a non-HWC layout (B200 addition: decoder-native NV12)
+  // frame columns the kernel also accepts in a non-HWC layout (an addition to the reference's API: decoder-native NV12)
   std::map<std::string, FrameLayout> input_layouts;
 };
 

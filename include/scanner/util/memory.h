@@ -3,7 +3,7 @@
 //   new_buffer / new_block_buffer / new_block_buffer_size / new_block_buffer_sizes allocate on a
 //   DeviceHandle; a "block" is one allocation carved into N element buffers sharing one
 //   refcount; add_buffer_ref(s) / delete_buffer adjust it by any pointer inside the block.
-// B200 design (not the reference's first-fit pool under a global mutex, memory.cpp:164-267):
+// This project's design (not the reference's first-fit pool under a global mutex, memory.cpp:164-267):
 //   GPU blocks come from a per-device stream-ordered CUDA memory pool (cudaMallocAsync on the
 //   device's pipeline stream, release threshold = unlimited so freed blocks are recycled without
 //   touching the driver); CPU blocks are pinned host memory when a GPU is present so every
@@ -63,7 +63,7 @@ void copy_or_ref_buffers(std::vector<u8*>& dest_buffers, DeviceHandle dest_devic
 u64 current_memory_allocated(DeviceHandle device);
 u64 max_memory_allocated(DeviceHandle device);
 
-// --- B200 additions -----------------------------------------------------------------------
+// --- additions to the reference's API -----------------------------------------------------------------------
 // The CUDA stream all engine-issued work for GPU `id` is ordered on (cudaStream_t as void*).
 // GPU kernels written against this API enqueue on it instead of the legacy default stream and
 // do NOT synchronise before returning: the engine orders consumers on the same stream and

@@ -2,7 +2,7 @@
  * scn_kernels.h -- C-ABI kernel layer of scanner-b200 (libscn_kernels.so).
  *
  * The thin layer the C++ host pipeline (and any foreign binding: ctypes, cgo, JNI ...) calls
- * to run the per-frame pixel ops of Scanner's decode->evaluate->save hot path on a B200.
+ * to run the per-frame pixel ops of Scanner's decode->evaluate->save hot path on an H100.
  * Plain pointers and sizes only -- no torch, no C++ types.  Each entry point names the
  * reference interface it replaces (paths relative to scanner-research/scanner @ 04a0c4b).
  *

@@ -1,7 +1,7 @@
 """ctypes loader for oracle/_ref/libref_image.so -- the reference's own scanner/util/image.cu,
 compiled unmodified by oracle/Makefile (`make -C oracle ref`).  TEST INFRASTRUCTURE ONLY: used by
-tests/test_ref_pin_gpu.py and oracle/make_golden_ref.py to pin the oracle and the CUDA kernels to
-what the reference's kernel computes on B200.  Needs a GPU; nothing under scanner_b200/ imports it.
+oracle/make_golden_ref.py to record what the reference's kernel computes, the golden data that pins the
+oracle and the CUDA kernels.  Needs a GPU; nothing under scanner_b200/ imports it.
 """
 import ctypes
 import os

@@ -1,5 +1,5 @@
 // C entry point over the reference's OWN H.264 byte-stream index creator -- test infrastructure.
-// oracle/Makefile compiles this with /root/reference/scanner/video/h264_byte_stream_index_creator.cpp (unmodified; it
+// oracle/Makefile compiles this with the reference's scanner/video/h264_byte_stream_index_creator.cpp (unmodified; it
 // parses with the reference's scanner/util/h264.h) into oracle/_ref/libref_h264_index.so.
 // tests/test_reference_h264_index_cpu.py feeds it the access units of the synthetic streams and compares frame count,
 // key pictures and sample sizes with this repo's indexer (scanner_b200/csrc/engine/h264.cpp).

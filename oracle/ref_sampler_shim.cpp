@@ -1,5 +1,5 @@
 // C entry points over the reference's OWN samplers and partitioners -- test infrastructure.
-// oracle/Makefile compiles this file together with /root/reference/scanner/engine/sampler.cpp (unmodified) into
+// oracle/Makefile compiles this file together with the reference's scanner/engine/sampler.cpp (unmodified) into
 // oracle/_ref/libref_sampler.so; tests/test_reference_samplers_cpu.py compares the engine's Sample / Space / Slice
 // row algebra with it on random arguments.  Interfaces used: DomainSampler (sampler.h:36-63), Partitioner (:75-103),
 // make_domain_sampler_instance (:66-69), make_partitioner_instance (:105-107).

@@ -202,12 +202,12 @@ ORC_API void orc_blur_u8c3(const uint8_t* src, int width, int height,
  *   B = Y'*1.1644 + Cb'*2.0172 + Cr'*0
  *   clamp to [0,1023], truncate to uint, >>2   (:92-102)
  * The reference is CUDA source compiled by nvcc with its default -fmad=true.
- * oracle/_ref builds that source UNMODIFIED (oracle/Makefile, nvcc 12.9, sm_100a);
+ * oracle/_ref builds that source UNMODIFIED (oracle/Makefile, nvcc 12.9, sm_90a);
  * its SASS evaluates `a*b + c*d + e*f` as  fma(e,f, fma(a,b, fl(c*d)))  -- the
  * MIDDLE product is the one rounded on its own (FMUL cb*k1; FFMA luma,k0; FFMA
  * cr,k2).  That order is written out explicitly here, and
- * tests/test_ref_pin_gpu.py runs the compiled reference kernel on B200 over all
- * 2^24 (Y,Cb,Cr) triples and asserts equality with this function.
+ * tests/golden/nv12_ref.npz holds that kernel's output over all 2^24 (Y,Cb,Cr)
+ * triples (run on an H100), and tests/test_oracle_golden.py asserts equality with this function.
  * (There is no -16 luma offset in the reference, :74.) */
 static inline uint8_t orc_pack10(float v) {
   v = fminf(fmaxf(v, 0.0f), 1023.f);

@@ -1,7 +1,7 @@
-"""scanner_b200 -- B200-native implementation of Scanner's decode -> evaluate -> save hot path.
+"""scanner_b200 -- H100-native implementation of Scanner's decode -> evaluate -> save hot path.
 
 Layers (see DESIGN.md):
-  include/scn_kernels.h + scanner_b200/csrc   hand-written sm_100a kernels behind a C ABI
+  include/scn_kernels.h + scanner_b200/csrc   hand-written sm_90a kernels behind a C ABI
   include/scanner/...   + scanner_b200/csrc/engine   C++ host pipeline with Scanner's
                                                      REGISTER_OP / REGISTER_KERNEL plugin API
   scanner_b200/*.py     thin Python surface (ctypes over the C ABI; scannerpy-shaped graph API)

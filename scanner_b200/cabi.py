@@ -57,7 +57,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise ScnError(
                 f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; "
-                "g.build()'` (nvcc, sm_100a). scanner_b200 has no CPU fallback.")
+                "g.build()'` (nvcc, sm_90a). scanner_b200 has no CPU fallback.")
         l = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(l, name)  # AttributeError if the .so lacks a declared symbol

@@ -1,4 +1,4 @@
-// blur.cu -- integer box filter on u8 HWC 3-channel frames (sm_100a).
+// blur.cu -- integer box filter on u8 HWC 3-channel frames (sm_90a).
 // Replaces BlurKernel::execute (reference tests/test_ops.cpp:265-294): for interior pixels
 // out = (sum of the (fl+fr+1)^2 window) / (fl+fr+1)^2 with fl = ceil(k/2)-1, fr = k/2; the
 // reference never writes the border of its freshly allocated frame -- here it is written as 0.
@@ -531,7 +531,7 @@ int launch_blur(const uint8_t* const* sp, int n, int width, int height, int ksiz
       const unsigned gx = (unsigned)((quads + out_quads * BP_WARPS - 1) / (out_quads * BP_WARPS));
       // rows per strip: a strip re-reads k - 1 rows of its neighbour; shorter strips when the grid would not fill the GPU
       int rows = 128;
-      while (rows > 32 && (size_t)gx * ((height + rows - 1) / rows) * cnt < 2 * 148) rows >>= 1;
+      while (rows > 32 && (size_t)gx * ((height + rows - 1) / rows) * cnt < 2 * (size_t)sm_count()) rows >>= 1;
       dim3 grid(gx, (unsigned)((height + rows - 1) / rows), (unsigned)cnt);
       LaunchScope ls("box_packed_kernel", st);
       switch (k) {

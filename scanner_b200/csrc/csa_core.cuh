@@ -1,4 +1,4 @@
-// csa_core.cuh -- bit-sliced counting primitives shared by the histogram kernels (sm_100a).
+// csa_core.cuh -- bit-sliced counting primitives shared by the histogram kernels (sm_90a).
 //   * PRMT as an 8-entry byte LUT: four 4-bit bins (the nibbles of a 16-bit selector) -> four
 //     one-hot bytes.  Word A carries bins 0..7 (bin 15 shows up as 0xFF through PRMT's
 //     sign-replicate mode), word B (selector ^ 0x8888) bins 8..14; bin 15 is recovered from the

@@ -1,6 +1,6 @@
 // digest.cu -- scn_frame_digest: 16-byte integer fingerprint of device buffers (include/scn_kernels.h).
 // Streaming read with 128-bit loads, 64-bit accumulators per thread, one warp-shuffle reduction and two
-// atomics per warp; grid = 148 x 4 CTAs striding over the words of all buffers.
+// atomics per warp; grid = 4 CTAs per SM striding over the words of all buffers.
 #include "scn_common.cuh"
 
 namespace scn {

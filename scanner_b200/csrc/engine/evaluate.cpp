@@ -444,6 +444,8 @@ Result EvaluateWorker::feed(std::map<i32, ColumnBatch>& source_columns,
           if (out[c].size() != nb) {
             RESULT_ERROR(&r, "Op %s produced %zu output elements for column %zu. Expected %zu outputs.",
                          op.name.c_str(), out[c].size(), c, nb);
+            // columns before c are already in `produced` (or freed); the rest are still the kernel's
+            for (size_t c2 = c; c2 < n_out; ++c2) delete_elements(st.out_dev[c2], out[c2]);
             return r;
           }
           if (an_.last_use[k][c] < 0) {  // unused output: free immediately (:1105-1114)

@@ -2,6 +2,7 @@
 // driver ABI (Video Codec SDK nvcuvid.h / cuviddec.h: field order and sizes, reserved tails kept
 // as opaque padding); only the fields this file touches are named.
 #include "nvdec.h"
+#include "swdec.h"
 
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -234,6 +235,54 @@ struct NvdecSession::Impl {
   i64* decoded_counter = nullptr;
   i64* used_counter = nullptr;
 
+  // software decode (no NVDEC engine on the GPU): pictures decoded by FFmpeg wait in host memory until advance()
+  // uploads each into `sw_surface` on the session stream and hands it to the consumer (stream order keeps the next
+  // upload behind the consumer's work)
+  std::unique_ptr<SwdecSession> sw;
+  std::deque<std::pair<i64, std::vector<u8>>> sw_pending;
+  u8* sw_surface = nullptr;
+  size_t sw_surface_bytes = 0;
+  int sw_width = 0, sw_height = 0;
+
+  Result sw_deliver() {
+    Result r;
+    const size_t bytes = (size_t)sw_width * sw_height * 3 / 2;
+    while (!sw_pending.empty()) {
+      auto& p = sw_pending.front();
+      if (bytes > sw_surface_bytes) {
+        if (sw_surface) {
+          cudaStreamSynchronize(stream);
+          cudaFree(sw_surface);
+        }
+        sw_surface = nullptr;
+        sw_surface_bytes = 0;
+        if (cudaMalloc((void**)&sw_surface, bytes) != cudaSuccess) {
+          RESULT_ERROR(&r, "software decode: cudaMalloc of %zu bytes failed", bytes);
+          return r;
+        }
+        sw_surface_bytes = bytes;
+      }
+      // from pageable memory: the call returns once the source has been staged, so the buffer may go
+      if (cudaMemcpyAsync(sw_surface, p.second.data(), bytes, cudaMemcpyHostToDevice, stream) != cudaSuccess) {
+        RESULT_ERROR(&r, "software decode: upload of a picture failed");
+        return r;
+      }
+      Nv12Surface s;
+      s.luma = sw_surface;
+      s.chroma = sw_surface + (size_t)sw_width * sw_height;
+      s.pitch = (size_t)sw_width;
+      s.width = sw_width;
+      s.height = sw_height;
+      {
+        ScopedNs t(3);
+        (*consumer)(p.first, s);
+      }
+      sw_pending.pop_front();
+    }
+    r.set_success(true);
+    return r;
+  }
+
   struct Mapped {
     unsigned long long dptr;
     cudaEvent_t done;
@@ -388,6 +437,10 @@ NvdecSession::~NvdecSession() {
   if (cuda_available()) {
     ScopedDevice sd(impl_->gpu);
     make_context_current(impl_->gpu);
+    if (impl_->sw_surface) {
+      cudaStreamSynchronize(impl_->stream);
+      cudaFree(impl_->sw_surface);
+    }
     impl_->release_all();
     if (impl_->decoder) driver().DestroyDecoder(impl_->decoder);
     if (impl_->parser) driver().DestroyVideoParser(impl_->parser);
@@ -395,12 +448,21 @@ NvdecSession::~NvdecSession() {
   }
 }
 
+bool NvdecSession::software() const { return impl_->sw != nullptr; }
+
 Result NvdecSession::init() {
   Result r;
   const NvdecCaps& caps = nvdec_caps(impl_->gpu);
   if (!caps.available || !caps.h264_supported) {
-    RESULT_ERROR(&r, "NVDEC unavailable on GPU %d: %s", impl_->gpu,
-                 caps.error.empty() ? "H.264 not supported" : caps.error.c_str());
+    impl_->sw.reset(new SwdecSession(1, true));
+    Result sr = impl_->sw->init();
+    if (!sr.success()) {
+      impl_->sw.reset();
+      RESULT_ERROR(&r, "NVDEC unavailable on GPU %d (%s) and no software decoder: %s", impl_->gpu,
+                   caps.error.empty() ? "H.264 not supported" : caps.error.c_str(), sr.msg().c_str());
+      return r;
+    }
+    r.set_success(true);
     return r;
   }
   ScopedDevice sd(impl_->gpu);
@@ -451,7 +513,7 @@ void nvdec_host_ns(long long out[6]) {
 Result NvdecSession::begin_interval(const u8* data, const std::vector<u64>& offsets,
                                     const std::vector<u64>& sizes, const std::vector<u8>& prefix,
                                     bool may_reorder, const std::vector<i64>& wanted, i64 out_base,
-                                    Consumer consumer) {
+                                    int width, int height, Consumer consumer) {
   Result r;
   Impl& s = *impl_;
   if (s.active) {
@@ -460,6 +522,23 @@ Result NvdecSession::begin_interval(const u8* data, const std::vector<u64>& offs
   }
   ScopedDevice sd(s.gpu);
   make_context_current(s.gpu);
+  if (s.sw) {
+    s.wanted_store = wanted;
+    s.consumer_store = std::move(consumer);
+    s.consumer = &s.consumer_store;
+    s.sw_pending.clear();
+    s.sw_width = width;
+    s.sw_height = height;
+    const size_t bytes = (size_t)width * height * 3 / 2;
+    Impl* ip = &s;
+    r = s.sw->begin_interval(data, offsets, sizes, prefix, may_reorder, wanted, out_base, width, height,
+                             [ip, bytes](i64 out_index) {
+                               ip->sw_pending.emplace_back(out_index, std::vector<u8>(bytes));
+                               return ip->sw_pending.back().second.data();
+                             });
+    s.active = r.success();
+    return r;
+  }
   s.wanted_store = wanted;
   s.wanted = &s.wanted_store;
   s.wanted_pos = 0;
@@ -490,7 +569,7 @@ Result NvdecSession::begin_interval(const u8* data, const std::vector<u64>& offs
   return r;
 }
 
-size_t NvdecSession::delivered() const { return impl_->wanted_pos; }
+size_t NvdecSession::delivered() const { return impl_->sw ? impl_->sw->delivered() : impl_->wanted_pos; }
 
 Result NvdecSession::advance(size_t count) {
   Result r;
@@ -513,6 +592,13 @@ Result NvdecSession::advance(size_t count) {
     std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
     ~Busy() { acc += std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count(); }
   } busy{busy_ns_};
+  if (s.sw) {
+    r = s.sw->advance(count);
+    frames_decoded_ = s.sw->frames_decoded();
+    frames_used_ = s.sw->frames_used();
+    if (!r.success()) return r;
+    return s.sw_deliver();
+  }
   while (s.wanted_pos < count) {
     if (s.next_sample < s.offsets.size() && s.next_sample < last_needed) {
       const size_t i = s.next_sample++;
@@ -549,6 +635,16 @@ Result NvdecSession::end_interval() {
   }
   ScopedDevice sd(s.gpu);
   make_context_current(s.gpu);
+  if (s.sw) {
+    Result a = s.sw->end_interval();
+    frames_decoded_ = s.sw->frames_decoded();
+    frames_used_ = s.sw->frames_used();
+    if (a.success()) a = s.sw_deliver();
+    s.sw_pending.clear();
+    s.active = false;
+    s.consumer = nullptr;
+    return a;
+  }
   Result a = advance(s.wanted_store.size());
   // always leave the parser flushed so the next interval starts clean
   if (!s.flushed) {

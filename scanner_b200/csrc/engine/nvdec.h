@@ -4,7 +4,7 @@
 // hard-disables, evaluate_worker.cpp:90-93) and the feeder/retriever threads of
 // scanner/video/decoder_automata.cpp:104-351.
 //
-// Design (B200: 7 NVDEC engines per GPU, cuvidGetDecoderCaps on the box):
+// Design (H100: 7 NVDEC engines per GPU, cuvidGetDecoderCaps at run time):
 //  * libnvcuvid / libcuda are resolved with dlopen at first use -- no SDK headers or link-time
 //    stubs; the handful of driver structs used are declared in nvdec.cpp from the public ABI.
 //  * No threads, no polling: cuvidParseVideoData runs its callbacks synchronously, so feeding a
@@ -15,6 +15,11 @@
 //    that stream), and unmapped only after a CUDA event recorded behind the consumer completes --
 //    up to kMaxMapped surfaces in flight, no cudaDeviceSynchronize per frame (reference :297).
 //  * Many sessions per GPU (one per pipeline instance) keep all NVDEC engines busy.
+//  * A GPU that exposes no NVDEC engine to the process (a container started without the driver's video
+//    capability: cuvidGetDecoderCaps fails) still decodes: the session runs FFmpeg's H.264 decoder on the host
+//    (swdec.h, as the reference's pipelines do), uploads each wanted picture's NV12 planes on the session stream
+//    and hands the consumer the same surface layout.  H.264 decoding is bit-exact, so the pictures are the ones
+//    NVDEC would deliver.  software() says which decoder a session uses; the engine reports it per instance.
 #pragma once
 #include <functional>
 #include <memory>
@@ -67,10 +72,11 @@ class NvdecSession {
   //   k-th, so samples are fed until the wanted pictures have come out (at most to the end of the
   //   interval) instead of stopping at the last wanted position;
   //   wanted: ascending 0-based positions (display order, relative to the first sample) of the
-  //   pictures to deliver; delivered picture k is passed to `consumer` as index out_base + k.
+  //   pictures to deliver; delivered picture k is passed to `consumer` as index out_base + k;
+  //   width / height: the picture size the stream index announces.
   Result begin_interval(const u8* data, const std::vector<u64>& offsets, const std::vector<u64>& sizes,
                         const std::vector<u8>& prefix, bool may_reorder, const std::vector<i64>& wanted,
-                        i64 out_base, Consumer consumer);
+                        i64 out_base, int width, int height, Consumer consumer);
   // Feed samples until at least `count` of the wanted pictures have been delivered (the decoder
   // may deliver more); flushes at the end of the interval.
   Result advance(size_t count);
@@ -83,6 +89,8 @@ class NvdecSession {
 
   i64 frames_decoded() const { return frames_decoded_; }
   i64 frames_used() const { return frames_used_; }
+  // true: no NVDEC engine on this GPU, the session decodes with FFmpeg on the host
+  bool software() const;
   // host nanoseconds this session has spent feeding samples (cuvidParseVideoData with its decode /
   // map callbacks: waiting for the NVDEC engine); frames_decoded / busy = the session's picture rate
   i64 busy_ns() const { return busy_ns_; }

@@ -292,8 +292,8 @@ void TaskOutput::release() {
 
 // Run the calling thread on the CPUs that are local to `gpu` (its PCIe root's NUMA node,
 // /sys/bus/pci/devices/<bdf>/local_cpulist) intersected with what the process may use.  A decode
-// thread spends its life in cuvidMapVideoFrame waiting for doorbells from that GPU; on the two-socket
-// hosts of the B200 boxes a thread on the far socket adds a cross-socket hop to every wake-up.
+// thread spends its life in cuvidMapVideoFrame waiting for doorbells from that GPU; on a two-socket
+// host a thread on the far socket adds a cross-socket hop to every wake-up.
 // SCN_PIN_NUMA=0 disables.  Returns the number of CPUs in the mask (0: left alone).
 static int pin_thread_to_gpu_numa(i32 gpu) {
   const char* e = getenv("SCN_PIN_NUMA");
@@ -520,7 +520,7 @@ void Engine::instance_main(Instance* inst) {
                 else
                 r = hw->begin_interval(
                     st.encoded.data(), offs, szs, st.index.metadata_packets, st.index.may_reorder, iv.wanted, iv.out_base,
-                    [cur = &c, rsp = &rs, stream, w, h](i64 out_index, const Nv12Surface& s) {
+                    (int)w, (int)h, [cur = &c, rsp = &rs, stream, w, h](i64 out_index, const Nv12Surface& s) {
                       const u8* lp = s.luma;
                       const u8* cp = s.chroma;
                       u8* dst = cur->slot(out_index);
@@ -876,7 +876,7 @@ Result Engine::decode_rows(InputStream& stref, const std::vector<i64>& rows, i32
       std::vector<u64> offs(st->index.sample_offsets.begin() + iv.kf_start, st->index.sample_offsets.begin() + iv.kf_end);
       std::vector<u64> szs(st->index.sample_sizes.begin() + iv.kf_start, st->index.sample_sizes.begin() + iv.kf_end);
       r = sess.begin_interval(st->encoded.data(), offs, szs, st->index.metadata_packets, st->index.may_reorder, iv.wanted,
-                              iv.out_base,
+                              iv.out_base, (int)w, (int)h,
                               [&, w, h, fb](i64 out_index, const Nv12Surface& s) {
                                 const u8* lp = s.luma;
                                 const u8* cp = s.chroma;
@@ -1185,7 +1185,7 @@ Result Engine::run(Graph& graph, const std::vector<Job*>& jobs, i32 wps, i32 ios
         const std::vector<u64> offs(st->index.sample_offsets.begin(), st->index.sample_offsets.begin() + 1);
         const std::vector<u64> szs(st->index.sample_sizes.begin(), st->index.sample_sizes.begin() + 1);
         Result pr = sess->begin_interval(st->encoded.data(), offs, szs, st->index.metadata_packets, false, {0}, 0,
-                                         [](i64, const Nv12Surface&) {});
+                                         st->index.width, st->index.height, [](i64, const Nv12Surface&) {});
         if (pr.success()) pr = sess->advance(1);
         if (pr.success()) pr = sess->end_interval();
         sess->drain();
@@ -1241,8 +1241,7 @@ Result Engine::run(Graph& graph, const std::vector<Job*>& jobs, i32 wps, i32 ios
   stats_.counters["halo_exchange_us"] = rs.halo_ns / 1000;
   // per pipeline instance (= per decode session): what it decoded and how long it waited on its NVDEC
   // engine -- frames / busy is the session's picture rate, the evidence for where an end-to-end
-  // number below the expected one went (measured: all sessions of a run always share one rate, slow
-  // runs are slow for every session -- profiles/r02_e2e_variance.md)
+  // number below the expected one went
   for (size_t i = 0; i < instances.size(); ++i) {
     const Instance& in = *instances[i];
     const std::string k = "inst" + std::to_string(i) + "_";
@@ -1252,6 +1251,11 @@ Result Engine::run(Graph& graph, const std::vector<Job*>& jobs, i32 wps, i32 ios
     stats_.counters[k + "decode_busy_us"] = in.decode_busy_ns / 1000;
     stats_.counters[k + "wall_us"] = in.wall_ns / 1000;
   }
+  // GPU decode sessions that run FFmpeg on the host because the GPU exposes no NVDEC engine (nvdec.h)
+  i64 software_sessions = 0;
+  for (const auto& sl : slots_)
+    for (const auto& kv : sl->sessions) software_sessions += kv.second->software() ? 1 : 0;
+  stats_.counters["gpu_software_decode_sessions"] = software_sessions;
   stats_.interval_ns = rs.profiler.interval_totals_ns();
   stats_.interval_counts = rs.profiler.interval_counts();
   for (const Profiler::TaskRecord& rec : rs.profiler.records()) {

@@ -32,6 +32,7 @@ struct AvFrameHead {
   int format;
 };
 constexpr int kCodecH264 = 27, kPixRgb24 = 2, kSwsBicubic = 4, kLogPanic = 0;
+constexpr int kPixYuv420p = 0, kPixYuvj420p = 12;  // AV_PIX_FMT_YUV420P, AV_PIX_FMT_YUVJ420P
 constexpr int kErrAgain = -11;
 constexpr int kErrEof = -(int)((unsigned)'E' | ((unsigned)'O' << 8) | ((unsigned)'F' << 16) | ((unsigned)' ' << 24));
 
@@ -195,6 +196,7 @@ const SwdecCaps& swdec_caps() { return ffmpeg().caps; }
 
 struct SwdecSession::Impl {
   int threads = 1;
+  bool nv12 = false;       // deliver the decoded 4:2:0 planes as NV12 instead of RGB24
   void* ctx = nullptr;     // AVCodecContext
   void* packet = nullptr;  // AVPacket
   void* frame = nullptr;   // AVFrame
@@ -242,6 +244,30 @@ struct SwdecSession::Impl {
           f.frame_unref(frame);
           return -1;
         }
+        if (nv12) {
+          // 8-bit 4:2:0 planes as decoded: luma rows, then Cb / Cr interleaved (what an NVDEC surface holds)
+          u8* dst = dest(out_base + (i64)wanted_pos);
+          if (!dst || (fh->format != kPixYuv420p && fh->format != kPixYuvj420p)) {
+            error = "software decode to NV12: unsupported pixel format " + std::to_string(fh->format);
+            f.frame_unref(frame);
+            return -1;
+          }
+          for (int y = 0; y < height; ++y) memcpy(dst + (size_t)y * width, fh->data[0] + (size_t)y * fh->linesize[0], width);
+          u8* c = dst + (size_t)width * height;
+          for (int y = 0; y < height / 2; ++y) {
+            const u8* cb = fh->data[1] + (size_t)y * fh->linesize[1];
+            const u8* cr = fh->data[2] + (size_t)y * fh->linesize[2];
+            u8* row = c + (size_t)y * width;
+            for (int x = 0; x < width / 2; ++x) {
+              row[2 * x] = cb[x];
+              row[2 * x + 1] = cr[x];
+            }
+          }
+          ++wanted_pos;
+          ++used_count;
+          f.frame_unref(frame);
+          continue;
+        }
         if (!sws || sws_w != width || sws_h != height || sws_fmt != fh->format) {
           if (sws) f.sws_free_context(sws);
           // reference software_video_decoder.cpp:188-192: same size, -> RGB24, SWS_BICUBIC
@@ -271,7 +297,10 @@ struct SwdecSession::Impl {
   }
 };
 
-SwdecSession::SwdecSession(int threads) : impl_(new Impl()) { impl_->threads = threads < 1 ? 1 : threads; }
+SwdecSession::SwdecSession(int threads, bool nv12) : impl_(new Impl()) {
+  impl_->threads = threads < 1 ? 1 : threads;
+  impl_->nv12 = nv12;
+}
 SwdecSession::~SwdecSession() {}
 
 Result SwdecSession::init() {

@@ -10,8 +10,8 @@
 //                    (scanner_b200/engine.py points it at the FFmpeg build that ships inside the image's
 //                    opencv-python-headless wheel when the variable is unset), else
 //   the system's libavcodec.so.{62..58} / libavutil / libswscale through the normal search path.
-// Without them a CPU instance that is handed an H.264 source fails with an error that says so; GPU instances never
-// come here (NVDEC, nvdec.h).
+// Without them a CPU instance that is handed an H.264 source fails with an error that says so.  GPU instances decode
+// with NVDEC (nvdec.h); on a GPU that exposes no NVDEC engine to the process their NvdecSession decodes here, to NV12.
 //
 // No frame pool / queue threads (reference :45-46): avcodec_send_packet / avcodec_receive_frame are called from the
 // pipeline instance's own thread and every wanted picture is scaled straight into its element's memory.
@@ -37,10 +37,12 @@ const SwdecCaps& swdec_caps();
 
 class SwdecSession {
  public:
-  // dest(out_index) -> where the packed RGB24 picture (width * height * 3 bytes, rows `width * 3` apart) goes
+  // dest(out_index) -> where the packed RGB24 picture (width * height * 3 bytes, rows `width * 3` apart) goes; with
+  // nv12 the packed NV12 picture (width * height luma bytes, then height / 2 rows of interleaved Cb Cr, rows `width`
+  // apart: the decoded planes unconverted)
   using Dest = std::function<u8*(i64)>;
 
-  explicit SwdecSession(int threads = 1);
+  explicit SwdecSession(int threads = 1, bool nv12 = false);
   ~SwdecSession();
   Result init();
 

@@ -1,4 +1,4 @@
-// flow.cu -- dense optical flow of the reference's OpticalFlow op on the GPU (sm_100a).
+// flow.cu -- dense optical flow of the reference's OpticalFlow op on the GPU (sm_90a).
 // Replaces OpticalFlowKernelCPU::execute (reference tests/test_ops.cpp:63-111):
 //   gray = cvtColor(frame, COLOR_BGR2GRAY)                           (15-bit fixed point)
 //   flow = cv::FarnebackOpticalFlow(3, 0.5, false, 15, 3, 5, 1.2, 0)->calc(gray0, gray1)
@@ -141,7 +141,7 @@ constexpr int UMW = 32, UMH = 8;
 // Layout: the 5 expansion coefficients (R0, R1) and the 5 matrix elements (M) of a level are PLANES of w x h floats,
 // coefficient c of pixel (x, y) at [c * w * h + y * w + x].  With the 5 values of a pixel adjacent (20 bytes: no
 // 128-bit access possible) every one of the 30 loads / stores of a pixel here touched 5-6 cache lines per warp and the
-// kernel ran against the L1 wavefront rate (32 us at 1080p for 115 MB, profiles/r02_flow.md); planes make each a
+// kernel ran against the L1 wavefront rate; planes make each a
 // contiguous 128-byte row segment.
 __global__ void update_matrices_kernel(const float* __restrict__ R0, const float* __restrict__ R1,
                                        const float* __restrict__ flow, int w, int h, float* __restrict__ M) {
@@ -457,8 +457,7 @@ box_solve_fused_kernel(const float* __restrict__ M, int w, int h, double scale, 
 // Tile 88 x 32 outputs: 5 * (88 + 14) = 510 column-channels ~ 2 x 256 threads.  A thread takes a column-channel
 // and loads its 32 + 14 input rows ONCE into registers (coalesced: consecutive threads, consecutive floats), then
 // forms the 32 vertical window sums from them -- the first version re-read 18 rows for every 4 outputs through an
-// L1 squeezed by the shared-memory carve-out and was L2-bound (ncu: 490 MB of L2 traffic per 1080p launch for a
-// 41 MB input, 7.5 TB/s; profiles/r02_flow.md).
+// L1 squeezed by the shared-memory carve-out and was L2-bound (about 12x the input in L2 traffic per launch).
 constexpr int B32W = 88, B32H = 32;
 template <int MW>
 struct Box32Geom {

@@ -106,8 +106,7 @@ nv12_resize_kernel(PtrBatch lumas, PtrBatch chromas, size_t pitch, int width, in
     o[2] = (uint8_t)((a.b + b.b + c.b + d.b + 2) >> 2);
     return;
   }
-  // ncu (profiles/r02_nv12_resize.md): 300 instructions per destination pixel, issue-active 75 %, ALU pipe 69 % --
-  // instruction-bound.  Two leaner-looking forms were measured and were not faster: the XU-converting tap chain of
+  // Instruction-bound: four exact NV12 -> RGB conversions per destination pixel.  Two leaner-looking forms were measured and were not faster: the XU-converting tap chain of
   // nv12_stream.cuh (46 us instead of 37 us per 64 frames) and a row-organised kernel (a CTA per destination row,
   // uniform row addresses, u16 chroma loads, chroma terms computed once per sample, mulhi blend: 312 static
   // instructions, the same 37 us).
@@ -201,7 +200,7 @@ extern "C" int scn_nv12_hist_resize(const uint8_t* const* host_luma_ptrs,
     const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
     stream_ok = nvs::eligible(host_luma_ptrs + i0, host_chroma_ptrs + i0, cnt, pitch, width, height);
   }
-  // How Histogram + Resize of the same surfaces run (SCN_NV12_RESIZE, measured in profiles/r02_nv12_stream.md):
+  // How Histogram + Resize of the same surfaces run (SCN_NV12_RESIZE):
   //   fused    the Resize rows are produced inside the streaming pass (one HBM read of the surface);
   //   split    streaming histogram kernel, then nv12_resize_kernel behind it on the same stream;
   //   overlap  nv12_resize_kernel on a side stream next to the streaming kernel.

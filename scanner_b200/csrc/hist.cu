@@ -1,4 +1,4 @@
-// hist.cu -- 16-bin x 3-channel histogram of u8 HWC frames (sm_100a).
+// hist.cu -- 16-bin x 3-channel histogram of u8 HWC frames (sm_90a).
 // Replaces HistogramKernelCPU::execute (reference tests/test_ops.cpp:19-49): bin = v >> 4 per
 // channel, int32[3][16] channel-major per frame.  Integer, bit-exact.
 //

@@ -1,4 +1,4 @@
-// hist_csa.cuh -- bit-sliced streaming histogram for large u8 HWC 3-channel frames (sm_100a).
+// hist_csa.cuh -- bit-sliced streaming histogram for large u8 HWC 3-channel frames (sm_90a).
 //
 // Why: a 16-bin histogram at HBM speed needs ~25 bytes/clk/SM; shared-memory atomics manage ~1 and
 // per-byte register counters ~8 (integer pipe: 64 lanes/clk/SM).  Here (csa_core.cuh) PRMT turns

@@ -1,4 +1,4 @@
-// nv12.cu -- NV12 decoder surface -> dense RGB24 (sm_100a).
+// nv12.cu -- NV12 decoder surface -> dense RGB24 (sm_90a).
 // Replaces convertNV12toRGBA / NV12_to_RGB (reference scanner/util/image.cu:109-200,229-239).
 // The reference kernel does scalar byte loads and six scalar byte stores per thread; here one
 // thread converts 4 horizontally adjacent pixels: one 32-bit luma load, one 32-bit chroma load

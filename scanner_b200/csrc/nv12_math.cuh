@@ -3,7 +3,7 @@
 //   Y' = Y<<2, C' = (C<<2)-512 (10-bit widen), float matrix {1.1644,0,1.596; 1.1644,-.3918,
 //   -.813; 1.1644,2.0172,0}, clamp [0,1023], truncate, >>2.  On odd luma rows (except the last
 //   chroma row) chroma is the rounded average of the two neighbouring chroma rows (:133-151).
-// The products are contracted the way nvcc (12.9, default -fmad, sm_100a) contracts the reference
+// The products are contracted the way nvcc (12.9, default -fmad) contracts the reference
 // source `y*k0 + cb*k1 + cr*k2` -- read off the SASS of the unmodified image.cu (oracle/_ref):
 //     fma(cr, k2, fma(y, k0, fl(cb * k1)))          the MIDDLE product is rounded on its own.
 // Terms with a zero coefficient are dropped (x + (+-0) == x, and fl(y*k0 + (+-0)) == fl(y*k0)).

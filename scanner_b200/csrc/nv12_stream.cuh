@@ -3,9 +3,8 @@
 // with the reference's NV12->RGB arithmetic (scanner/util/image.cu:67-200 as nvcc contracts it, see
 // nv12_math.cuh) and neither the RGB frame nor a second read of the surface in HBM.
 //
-// Design (profiles/r02_pipe_ubench.md has the measured pipe model it is built on: a warp instruction
-// costs one issue slot; ALU-pipe LOP3/PRMT and FMA-pipe IMAD/FFMA2 occupy their 16-lane pipe for two
-// clocks, scalar FFMA one clock, XU conversions eight, and the pipes overlap):
+// Design (the kernel is bound by instruction issue, not by HBM: every choice below trades ALU, FMA and
+// XU (conversion) pipe work against each other so that no pipe is the only busy one):
 //   * surfaces are streamed with cp.async into a per-warp shared-memory ring (no load registers, the
 //     prefetch runs kStages-1 steps ahead across span and frame boundaries); a lane owns a "unit" of
 //     16 pixels x 2 rows per step (two luma rows, the chroma row and the next chroma row);
@@ -26,7 +25,6 @@
 //   * Resize: when a warp has finished the histogram of a span of rows it produces the destination
 //     rows whose first tap row starts in that span -- the taps were streamed moments ago and come
 //     from L1/L2, so the surface crosses HBM once.
-// Per 32-pixel step and lane: ~200 ALU, ~300 FMA-pipe, 32-64 XU instructions, ~600 issue slots.
 #pragma once
 #include "csa_core.cuh"
 #include "nv12_math.cuh"
@@ -75,26 +73,19 @@ constexpr float kQScale = 0.0625f;
 constexpr float kQBias = 0.0625f - 524288.0f;           // 1/16 - 2^19
 constexpr float kSInit = kMagic - 4369.0f;              // 2^23 - 0x1111
 
-using f2 = unsigned long long;  // two floats in an aligned register pair
-__device__ __forceinline__ f2 pack2(float lo, float hi) {
-  f2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
+// Two floats that take the same operation.  sm_90 has no packed f32x2 arithmetic: each helper is two
+// scalar instructions with the rounding of the packed form, so the results are bit-identical to it.
+struct f2 {
+  float lo, hi;
+};
+__device__ __forceinline__ f2 pack2(float lo, float hi) { return f2{lo, hi}; }
 __device__ __forceinline__ void unpack2(f2 v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
+  lo = v.lo;
+  hi = v.hi;
 }
 __device__ __forceinline__ f2 splat(float v) { return pack2(v, v); }
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) {
-  f2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ f2 fma2_rm(f2 a, f2 b, f2 c) {
-  f2 r;
-  asm("fma.rm.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
+__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return f2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)}; }
+__device__ __forceinline__ f2 fma2_rm(f2 a, f2 b, f2 c) { return f2{__fmaf_rd(a.lo, b.lo, c.lo), __fmaf_rd(a.hi, b.hi, c.hi)}; }
 __device__ __forceinline__ float fma_sat(float a, float b, float c) {
   float r;
   asm("fma.rn.sat.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
@@ -109,16 +100,8 @@ template <int K>
 __device__ __forceinline__ float byte_f(uint32_t w) {  // I2F.U8 Rd, Rs.BK (XU pipe)
   return (float)((w >> (8 * K)) & 0xFFu);
 }
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) {
-  f2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f2 add2(f2 a, f2 b) {
-  f2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return f2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ f2 add2(f2 a, f2 b) { return f2{__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
 
 // The two (Cb,Cr) samples of a chroma word, everything that does not depend on luma, as register
 // pairs (sample 0, sample 1) so that one packed instruction serves both

@@ -1,7 +1,7 @@
 // stdlib_ops.cu -- the per-frame ops of the hot path as a Scanner op plugin (libscn_stdlib.so).
 // Same op names, columns and argument messages as the reference's in-tree ops
 // (tests/test_ops.cpp:13-59 Histogram, :114-170 Resize, :239-310 Blur) -- but the kernels are
-// registered for DeviceType::GPU and run the sm_100a kernels of libscn_kernels.so on the
+// registered for DeviceType::GPU and run the sm_90a kernels of libscn_kernels.so on the
 // pipeline instance's stream.  Loaded with dlopen like any user op library (Client.load_op).
 #include <map>
 

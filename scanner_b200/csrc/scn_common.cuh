@@ -1,4 +1,4 @@
-// scn_common.cuh -- shared helpers for the sm_100a kernels behind include/scn_kernels.h.
+// scn_common.cuh -- shared helpers for the sm_90a kernels behind include/scn_kernels.h.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -43,9 +43,9 @@ struct LaunchScope {
 inline int sm_count() {
   static int sms = [] {
     int dev = 0, v = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0)
-      return 148;
+      return 132;
     return v;
   }();
   return sms;

@@ -1,7 +1,7 @@
 """Torch-tensor convenience wrappers over the C ABI (tests / bench / the Python op surface).
 
 torch is used only for device memory and streams; every function below enqueues hand-written
-sm_100a kernels from libscn_kernels.so on the current torch CUDA stream.
+sm_90a kernels from libscn_kernels.so on the current torch CUDA stream.
 """
 import ctypes
 

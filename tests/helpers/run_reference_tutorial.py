@@ -6,7 +6,9 @@ What is substituted is only what the machine cannot provide: the module name (`s
 to scanner_b200), the example-video download (`util.download_video`, no network) and -- because this
 helper is for machines without a GPU, where H.264 cannot be decoded -- the video file itself, which
 becomes a raw-frame stream.  Everything else (ops, graph, run, save_mp4, delete) is the tutorial's
-own code.  Used by tests/test_reference_tutorials_cpu.py where /root/reference exists.
+own code.  Run it by hand on a tutorial of a reference checkout (01, 02 and 04 need no GPU op); the
+tutorial files cannot be stored in this repository, so no test runs it.  tests/test_tutorials_gpu.py replays the
+tutorials' bodies.
 """
 import os
 import runpy

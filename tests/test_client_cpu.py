@@ -191,7 +191,7 @@ def test_reference_tutorial_00_on_the_cpu_with_a_real_video(tmp_path):
     data, _ = synth_h264.write(320, 240, 20, gop=5, seed=1)
     mp4 = str(tmp_path / "a.mp4")
     open(mp4, "wb").write(E.mp4_mux(data, 30, 1))
-    cl = Client(db_path=str(tmp_path / "db"))
+    cl = Client(gpus=[], db_path=str(tmp_path / "db"))   # CPU instances only, also where a GPU is present
     frames = cl.io.Input([NamedVideoStream(cl, "clip", path=mp4)])
     hist = cl.ops.Histogram(frame=frames, device=DeviceType.CPU)
     out = NamedStream(cl, "hists")

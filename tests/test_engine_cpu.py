@@ -261,6 +261,14 @@ def test_errors(eng):
     g3.add_sink((g3.add_op("TestWindow", [(s3, "nope")]), "window"))
     with pytest.raises(E.EngineError, match="does not have the requested column"):
         eng.run(g3, [j], 2, 2)
+    # the failed runs released what their kernels produced
+    g4 = E.Graph()
+    s4 = g4.add_source(False)
+    g4.add_sink((s4, "column"))
+    j4 = E.Job()
+    j4.bind_source(s4, eng.add_bytes(i64_rows(2)))
+    eng.run(g4, [j4], 2, 2)
+    assert eng.stats()["counters"]["cpu_bytes_live"] == 0
 
 
 # ------------------------------------------------------------------------------------------------

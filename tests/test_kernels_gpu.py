@@ -1,4 +1,4 @@
-"""Parity of the sm_100a kernels (called through the C ABI) against the oracle and the
+"""Parity of the sm_90a kernels (called through the C ABI) against the oracle and the
 committed golden vectors.  Integer / byte work: every comparison is bit-exact."""
 import os
 

@@ -131,15 +131,20 @@ def test_flow_1080p_matches_cv2_run_here():
 
 def test_nv12_matches_the_reference_kernels_own_output(golden_dir):
     """tests/golden/nv12_ref.npz holds what the reference's OWN kernel (scanner/util/image.cu compiled
-    unmodified, oracle/_ref) produced on a B200 (oracle/make_golden_ref.py): seeded surfaces, and the
-    SHA-256 of its output over an input set that presents every (Y,Cb,Cr) triple (synth.nv12_exhaustive).
-    The restatement must reproduce both -- this is what pins the oracle's FMA contraction order."""
+    unmodified, oracle/_ref) produced on an H100 (oracle/make_golden_ref.py): seeded surfaces (the output, or its
+    SHA-256 where it is large), and the SHA-256 of its output over an input set that presents every (Y,Cb,Cr) triple
+    (synth.nv12_exhaustive).  The restatement must reproduce both -- this is what pins the oracle's FMA contraction
+    order."""
     import hashlib
     g = np.load(os.path.join(golden_dir, "nv12_ref.npz"))
     for k in _cases(g):
         seed, h, w, pitch = [int(x) for x in g[k + "_meta"]]
         luma, chroma = synth.nv12_surface(seed, h, w, pitch)
-        assert (oracle.nv12_to_rgb(luma, chroma, w) == g[k + "_out"]).all(), (k, h, w, pitch)
+        got = oracle.nv12_to_rgb(luma, chroma, w)
+        if k + "_out" in g.files:
+            assert (got == g[k + "_out"]).all(), (k, h, w, pitch)
+        else:
+            assert hashlib.sha256(got.tobytes()).digest() == g[k + "_sha256"].tobytes(), (k, h, w, pitch)
     sha = hashlib.sha256()
     for f in range(synth.EXH_FRAMES):
         luma, chroma = synth.nv12_exhaustive(f)

@@ -1,25 +1,31 @@
 """This repo's H.264 indexer (scanner_b200/csrc/engine/h264.cpp) against the reference's OWN index creator.
 
-oracle/_ref/libref_h264_index.so is /root/reference/scanner/video/h264_byte_stream_index_creator.cpp compiled
+oracle/_ref/libref_h264_index.so is the reference's scanner/video/h264_byte_stream_index_creator.cpp compiled
 UNMODIFIED (with the reference's scanner/util/h264.h SPS / PPS / slice-header parsers and is_new_access_unit) behind a
 C shim.  The reference is fed what its demuxer would give it -- one packet per access unit, here the samples this
 repo's indexer cut out of the stream -- and must count exactly one new frame per packet (a sample that held two access
 units, or half of one, would not), name the same key pictures and the same sample sizes.  On a key picture the reference
 additionally writes a copy of every SPS / PPS it has seen in front of the packet, each with the 3 bytes before and
 after the NAL (:135-139, :193-214): sizes differ there by exactly that amount.
-Skipped where the library was not built (no /root/reference)."""
+The reference's answers are replayed from tests/golden/ref_h264_index.json; where oracle/_ref is built,
+`python tests/test_reference_h264_index_cpu.py` runs the library itself and records them again."""
 import ctypes
+import hashlib
 import os
+import sys
 
 import numpy as np
 import pytest
 
-from scanner_b200 import engine as E
-from scanner_b200 import synth_h264
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from oracle.recorded import Answers  # noqa: E402
+from scanner_b200 import engine as E  # noqa: E402
+from scanner_b200 import synth_h264  # noqa: E402
+
 REF_SO = os.path.join(ROOT, "oracle", "_ref", "libref_h264_index.so")
-pytestmark = pytest.mark.skipif(not os.path.exists(REF_SO), reason="oracle/_ref/libref_h264_index.so not built")
+REF = Answers("ref_h264_index")
 
 
 def nal_units(buf):
@@ -53,7 +59,7 @@ def my_index(tmp_path, name, stream):
     return data, list(vd.sample_offsets), list(vd.sample_sizes), list(vd.keyframe_indices)
 
 
-def reference_index(data, offs, sizes):
+def live_reference_index(data, offs, sizes):
     lib = ctypes.CDLL(REF_SO)
     n = len(offs)
     UL = ctypes.c_ulong
@@ -66,7 +72,11 @@ def reference_index(data, offs, sizes):
     rc = lib.ref_h264_index(buf, (UL * n)(*offs), (UL * n)(*sizes), n, so, ss, kf, n + 8, ctypes.byref(nf), ctypes.byref(nk),
                             out, UL(cap), ctypes.byref(slen), err, 256)
     assert rc == 0, err.value
-    return nf.value, list(so[:nf.value]), list(ss[:nf.value]), list(kf[:nk.value]), bytes(out[:slen.value])
+    nfv, stream = nf.value, bytes(out[:slen.value])
+    so, ss = list(so[:nfv]), list(ss[:nfv])
+    # recorded: the demuxed stream's SHA-256 and the bytes the reference wrote in front of each sample
+    inserted = [stream[so[i]:so[i] + max(0, ss[i] - sizes[i])] for i in range(nfv)]
+    return [nfv, so, ss, list(kf[:nk.value]), hashlib.sha256(stream).hexdigest(), inserted]
 
 
 def streams():
@@ -84,7 +94,10 @@ def test_indexer_agrees_with_the_reference_index_creator(tmp_path, case):
     name, stream, n = case
     data, offs, sizes, keys = my_index(tmp_path, name, stream)
     assert len(offs) == n
-    frames, r_offs, r_sizes, r_keys, r_stream = reference_index(data, offs, sizes)
+    frames, r_offs, r_sizes, r_keys, r_sha, inserted = REF(data, offs, sizes)
+    # the reference's demuxed stream: what it wrote in front of each sample, then the sample (held by its SHA-256)
+    r_stream = b"".join(inserted[i] + data[offs[i]:offs[i] + sizes[i]] for i in range(min(frames, n)))
+    assert hashlib.sha256(r_stream).hexdigest() == r_sha
     assert frames == n                       # every sample is exactly one access unit for the reference's parser
     assert r_keys == keys                    # the same key pictures (IDR access units)
     # parameter sets the reference has seen so far, as it copies them: NAL + 3 bytes on each side
@@ -103,3 +116,14 @@ def test_indexer_agrees_with_the_reference_index_creator(tmp_path, case):
     # with the inserted copies taken out again the reference's demuxed stream is the stream this repo stores
     rebuilt = b"".join(r_stream[r_offs[i] + extra_by_frame.get(i, 0):r_offs[i] + r_sizes[i]] for i in range(n))
     assert rebuilt == data
+
+
+if __name__ == "__main__":
+    import pathlib
+    import tempfile
+    REF = Answers("ref_h264_index", live_reference_index)
+    for c in streams():
+        with tempfile.TemporaryDirectory() as d:
+            test_indexer_agrees_with_the_reference_index_creator(pathlib.Path(d), c)
+    REF.save()
+    print("wrote", REF.path, len(REF.table), "answers")

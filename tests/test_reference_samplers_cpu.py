@@ -1,55 +1,85 @@
 """The engine's Sample / Space / Slice row algebra against the reference's OWN samplers and partitioners.
 
-oracle/_ref/libref_sampler.so is /root/reference/scanner/engine/sampler.cpp compiled UNMODIFIED (oracle/Makefile) behind
+oracle/_ref/libref_sampler.so is the reference's scanner/engine/sampler.cpp compiled UNMODIFIED (oracle/Makefile) behind
 a C shim (oracle/ref_sampler_shim.cpp).  For random arguments the rows a pipeline `source -> Sample/Space -> sink`
 produces in this engine (values = the source row each output row carries, None = null row) must be what the
 reference's get_num_downstream_rows / get_downstream_rows say for the full input, and the Slice groups must be the
 reference partitioner's groups.  The argument bytes are the same proto3 wire bytes on both sides.
-Skipped where the library was not built (no /root/reference)."""
+The reference's answers are replayed from tests/golden/ref_samplers.json; where oracle/_ref is built,
+`python tests/test_reference_samplers_cpu.py` runs these tests against the library itself and records them again."""
 import ctypes
 import os
 import struct
 import subprocess
+import sys
 
 import numpy as np
 import pytest
 
-from scanner_b200 import engine as E
-from scanner_b200 import protolite
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from oracle.recorded import Answers  # noqa: E402
+from scanner_b200 import engine as E  # noqa: E402
+from scanner_b200 import protolite  # noqa: E402
+
 REF_SO = os.path.join(ROOT, "oracle", "_ref", "libref_sampler.so")
-pytestmark = pytest.mark.skipif(not os.path.exists(REF_SO), reason="oracle/_ref/libref_sampler.so not built")
 SA = protolite.SAMPLER_ARGS
 _L = ctypes.c_long
 
 
-@pytest.fixture(scope="module")
-def ref():
-    lib = ctypes.CDLL(REF_SO)
+def live_reference(lib):
+    """The reference library called through its shim: (kind, fn, args, x) -> the answer the tests record."""
     lib.ref_sampler_downstream.restype = _L
     lib.ref_sampler_upstream.restype = _L
     lib.ref_partitioner_groups.restype = _L
-    return lib
+
+    def call(kind, fn, args, x):
+        err = ctypes.create_string_buffer(512)
+        if kind == "downstream":
+            n = x
+            cap = 64 * n + 64
+            rows, mp, nd = (_L * cap)(), (_L * cap)(), _L(0)
+            k = lib.ref_sampler_downstream(fn.encode(), args, len(args), _L(n), rows, mp, ctypes.c_size_t(cap),
+                                           ctypes.byref(nd), err, ctypes.c_size_t(512))
+            assert k >= 0, (fn, err.value)
+            return [nd.value, list(rows[:k]), list(mp[:k])]
+        if kind == "upstream":
+            out, down = (_L * 64)(), (_L * len(x))(*x)
+            k = lib.ref_sampler_upstream(fn.encode(), args, len(args), down, ctypes.c_size_t(len(x)), out,
+                                         ctypes.c_size_t(64), None, ctypes.c_size_t(0))
+            return list(out[:k])
+        n = x
+        rows, offs = (_L * (8 * n + 64))(), (_L * 256)()
+        ng = lib.ref_partitioner_groups(fn.encode(), args, len(args), _L(n), rows, ctypes.c_size_t(8 * n + 64), offs,
+                                        ctypes.c_size_t(256), err, ctypes.c_size_t(512))
+        assert ng >= 0, (fn, err.value)
+        return [list(rows[offs[g]:offs[g + 1]]) for g in range(ng)]
+    return call
 
 
-@pytest.fixture(scope="module", autouse=True)
-def plugin():
+@pytest.fixture(scope="module")
+def ref():
+    return Answers("ref_samplers")
+
+
+def load_plugin():
     subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "liborc.so"], stdout=subprocess.DEVNULL)
     subprocess.check_call(["make", "-C", os.path.join(ROOT, "tests", "cpp")], stdout=subprocess.DEVNULL)
     if "TestWindow" not in E.list_ops():
         E.load_op_library(os.path.join(ROOT, "build", "tests", "libtest_plugin_ops.so"))
 
 
+@pytest.fixture(scope="module", autouse=True)
+def plugin():
+    load_plugin()
+
+
 def ref_downstream(ref, fn, args, n):
-    cap = 64 * n + 64
-    rows, mp = (_L * cap)(), (_L * cap)()
-    nd, err = _L(0), ctypes.create_string_buffer(512)
-    k = ref.ref_sampler_downstream(fn.encode(), args, len(args), _L(n), rows, mp, ctypes.c_size_t(cap), ctypes.byref(nd),
-                                   err, ctypes.c_size_t(512))
-    assert k >= 0, (fn, err.value)
+    nd, rows, mp = ref("downstream", fn, args, n)
+    k = len(rows)
     assert list(rows[:k]) == list(range(k)) or fn in ("Gather", "Strided", "StridedRanges", "All")
-    return nd.value, list(rows[:k]), list(mp[:k])
+    return nd, rows, mp
 
 
 def engine_rows(eng, n, fn, args, space):
@@ -109,11 +139,7 @@ def test_samplers_required_upstream_rows_agree(ref):
         _, _, m2 = ref_downstream(ref, "Gather", a2, n1)
         want = [m1[i] for i in m2]
         # the reference's own answer to "which rows of the Strided stream do these Gather rows need"
-        out = (_L * 64)()
-        down = (_L * len(pick))(*range(len(pick)))
-        k = ref.ref_sampler_upstream(b"Gather", a2, len(a2), down, ctypes.c_size_t(len(pick)), out, ctypes.c_size_t(64),
-                                     None, ctypes.c_size_t(0))
-        assert list(out[:k]) == pick
+        assert ref("upstream", "Gather", a2, list(range(len(pick)))) == pick
         g = E.Graph()
         src = g.add_source(False)
         s1 = g.add_sample((src, "column"))
@@ -151,11 +177,7 @@ def test_partitioners_agree_with_the_reference(ref):
         groups = [protolite.encode(SA["GatherList"], {"rows": rows_}) for rows_ in group_rows]
         cases.append(("Gather", protolite.encode(SA["GatherPartitionerArgs"], {"groups": groups}), n, group_rows))
     for fn, args, n, want_groups in cases:
-        rows, offs, err = (_L * (8 * n + 64))(), (_L * 256)(), ctypes.create_string_buffer(512)
-        ng = ref.ref_partitioner_groups(fn.encode(), args, len(args), _L(n), rows, ctypes.c_size_t(8 * n + 64), offs,
-                                        ctypes.c_size_t(256), err, ctypes.c_size_t(512))
-        assert ng >= 0, (fn, err.value)
-        ref_groups = [list(rows[offs[g]:offs[g + 1]]) for g in range(ng)]
+        ref_groups = ref("groups", fn, args, n)
         g = E.Graph()
         src = g.add_source(False)
         sl = g.add_slice((src, "column"))
@@ -180,3 +202,13 @@ def test_partitioners_agree_with_the_reference(ref):
         assert vals == [r for grp in ref_groups for r in grp], (fn, vals, ref_groups)       # rows, group after group
         assert cnts == [i for grp in ref_groups for i in range(len(grp))], (fn, cnts)          # state restarts per group
     eng.close()
+
+
+if __name__ == "__main__":
+    live = Answers("ref_samplers", live_reference(ctypes.CDLL(REF_SO)))
+    load_plugin()
+    test_samplers_agree_with_the_reference_on_random_arguments(live)
+    test_samplers_required_upstream_rows_agree(live)
+    test_partitioners_agree_with_the_reference(live)
+    live.save()
+    print("wrote", live.path, len(live.table), "answers")

@@ -33,7 +33,7 @@ def clip(seed, w, h, frames, gop=30):
 def inst(args, tuned):
     """pipeline instances per GPU: --instances, else the value tuned for the config (the reference's
     pipeline_instances_per_node knob): P_Skip-heavy 1080p decode is best at one session per NVDEC
-    engine (7), IDR-heavy or 4K decode at two (14); see profiles/r01_configs.md."""
+    engine (7), IDR-heavy or 4K decode at two (14)."""
     return args.instances if args.instances > 0 else tuned
 
 

@@ -1,12 +1,12 @@
 #!/usr/bin/env python3
 """Per-kernel measured-bytes roofline of the Farneback path from an ncu CSV log.
 
-On the GPU box:
+On a GPU:
   ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum,lts__t_bytes.sum,\
 smsp__issue_active.avg.pct_of_peak_sustained_active,smsp__inst_executed.sum --clock-control none \
-      -k regex:'gray|gauss|poly|resize_f32|update_matrices|box_' -c 200 --csv --log-file gpurun_out/flow_ncu.csv \
+      -k regex:'gray|gauss|poly|resize_f32|update_matrices|box_' -c 200 --csv --log-file flow_ncu.csv \
       python tools/flow_roofline.py drive
-Here:  python tools/flow_roofline.py table gpurun_out/flow_ncu.csv [peak GB/s] > profiles/...md
+Then:  python tools/flow_roofline.py table flow_ncu.csv [peak GB/s]
 `drive` runs 3 consecutive 1080p pairs of one clip (the op's access pattern; the first pair expands two frames).
 """
 import csv

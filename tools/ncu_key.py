@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Key numbers of an .ncu-rep (read here, no GPU): python tools/ncu_key.py profiles/x.ncu-rep"""
+"""Key numbers of an .ncu-rep (read here, no GPU): python tools/ncu_key.py x.ncu-rep"""
 import csv
 import subprocess
 import sys

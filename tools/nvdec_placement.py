@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """How do decode sessions land on the NVDEC engines, and does dropping slow sessions fix a bad placement?
 
-For `trials` fresh engines (7 pipeline instances = 7 decode sessions on one B200): four runs of the bench's
+For `trials` fresh engines (7 pipeline instances = 7 decode sessions on one H100): four runs of the bench's
 end-to-end workload (56 clips x 120 frames 1080p, GOP 30) each; per run the frames/s and every session's
 picture rate (frames decoded / host time spent waiting on its engine).  One JSON line per run.
 usage: python tools/nvdec_placement.py [trials]"""

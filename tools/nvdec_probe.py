@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Probe the GPU box for NVDEC: is libnvcuvid there, and what does cuvidGetDecoderCaps say for
-H.264 4:2:0 8-bit?  (SURVEY.md Appendix B: 'call it first on the GPU box'.)  Prints one JSON line."""
+"""Probe a GPU for NVDEC: is libnvcuvid there, and what does cuvidGetDecoderCaps say for
+H.264 4:2:0 8-bit?  (SURVEY.md Appendix B: 'call it first on the GPU'.)  Prints one JSON line."""
 import ctypes
 import glob
 import json

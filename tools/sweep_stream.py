@@ -3,7 +3,7 @@
 conversion pipe.
 
     python tools/sweep_stream.py build     # here (no GPU): build/variants/<tag>/libscn_kernels.so
-    python tools/sweep_stream.py run       # on the GPU box: time + check every variant, one JSON line each
+    python tools/sweep_stream.py run OUT   # on a GPU: time + check every variant, one JSON line each, all in OUT
 """
 import json
 import os
@@ -60,8 +60,7 @@ print(json.dumps(out))
 '''
 
 
-def run():
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
+def run(out_path):
     res = {}
     for build_tag, mode in RUNS:
         tag = f"{build_tag}_{mode}"
@@ -74,8 +73,8 @@ def run():
         except Exception:
             res[tag] = {"error": r.stdout[-400:]}
         print(tag, res[tag], flush=True)
-    json.dump(res, open(os.path.join(ROOT, "gpurun_out", "sweep_stream.json"), "w"), indent=1)
+    json.dump(res, open(out_path, "w"), indent=1)
 
 
 if __name__ == "__main__":
-    {"build": build, "run": run}[sys.argv[1]]()
+    build() if sys.argv[1] == "build" else run(sys.argv[2])
