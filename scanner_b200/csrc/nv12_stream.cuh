@@ -215,7 +215,7 @@ struct Params {
   size_t pitch;
   int width, height;
   uint32_t units_per_row;     // width / 16
-  uint32_t upr_recip;         // floor(2^32 / units_per_row) + 1
+  uint64_t upr_recip;         // floor(2^32 / units_per_row) + 1: 33 bits when units_per_row == 1
   uint32_t units_per_frame;   // units_per_row * height / 2
   uint32_t steps_per_frame;   // ceil(units_per_frame / 32)
   uint64_t total_steps;
@@ -381,7 +381,7 @@ nv12_stream_kernel(const Params prm, int32_t* __restrict__ out) {
   const uint8_t *pf_l, *pf_c;                              // its luma / chroma 16-byte groups
   auto locate = [&]() {
     pf_unit = pf_s * 32u + (uint32_t)lane;
-    pf_yp = __umulhi(pf_unit, prm.upr_recip);
+    pf_yp = (uint32_t)(((uint64_t)pf_unit * prm.upr_recip) >> 32);   // == pf_unit / units_per_row
     pf_xs = pf_unit - pf_yp * prm.units_per_row;
     const bool active = pf_unit < prm.units_per_frame;     // lanes past the frame's last unit: any valid address
     pf_l = prm.luma.p[pf_frame] + (active ? (size_t)(2 * pf_yp) * prm.pitch + (size_t)pf_xs * 16 : 0);
@@ -553,7 +553,7 @@ inline int launch(const uint8_t* const* lp, const uint8_t* const* cp, int n, siz
     p.width = width;
     p.height = height;
     p.units_per_row = (uint32_t)(width / 16);
-    p.upr_recip = (uint32_t)((1ull << 32) / p.units_per_row) + 1u;
+    p.upr_recip = (1ull << 32) / p.units_per_row + 1u;
     p.units_per_frame = p.units_per_row * (uint32_t)(height / 2);
     p.steps_per_frame = (p.units_per_frame + 31) / 32;
     p.total_steps = (uint64_t)cnt * p.steps_per_frame;

@@ -83,6 +83,18 @@ def test_bad_arguments_are_rejected_without_a_gpu():
     assert l.scn_nv12_to_rgb24(None, None, 8, 1, 7, 8, None, 24, None) == -1  # odd width
 
 
+def test_nv12_stream_unit_division_by_multiply_shift_is_exact():
+    """nv12_stream_kernel splits a unit index u (16 pixels x 2 rows) into row pair and column with
+    (u * (floor(2^32 / upr) + 1)) >> 32, upr = width / 16 (nvs::launch, nvs::Params::upr_recip).  Exhaustive over every
+    width the kernel takes up to 8192 and every unit index a frame up to 8192 rows tall reaches, padding lanes of the
+    last step included.  The multiplier needs 33 bits at width 16: truncated to 32 it is 1 and every quotient is 0."""
+    for upr in range(1, 8192 // 16 + 1):
+        m = np.uint64((1 << 32) // upr + 1)
+        v = np.arange(upr * (8192 // 2) + 32, dtype=np.uint64)
+        q = (v * m) >> np.uint64(32)
+        assert ((v - q * np.uint64(upr)) < np.uint64(upr)).all(), upr * 16
+
+
 def test_no_silent_cpu_fallback():
     """On a box without CUDA the torch wrappers must raise, not compute on the CPU."""
     import torch
