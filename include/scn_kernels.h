@@ -140,6 +140,33 @@ SCN_API int scn_nv12_hist_resize(const uint8_t* const* host_luma_ptrs,
                          void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * ConvertColor  (replaces scannertools' ConvertColor kernel: cv::cvtColor(frame, out, code) on
+ *                CV_8U frames).  Bit-exact vs cv2.cvtColor.  Codes, numbered in this order:
+ *   0 COLOR_RGB2GRAY      1 COLOR_BGR2GRAY        HxWx3 -> HxWx1
+ *   2 COLOR_RGB2YCrCb     3 COLOR_BGR2YCrCb       HxWx3 -> HxWx3
+ *   4 COLOR_RGB2HSV       5 COLOR_BGR2HSV         HxWx3 -> HxWx3 (hue 0..179)
+ *   6 COLOR_RGB2HSV_FULL  7 COLOR_BGR2HSV_FULL    HxWx3 -> HxWx3 (hue 0..255)
+ *   8 COLOR_RGB2BGR       9 COLOR_BGR2RGB         HxWx3 -> HxWx3
+ *  10 COLOR_GRAY2RGB     11 COLOR_GRAY2BGR        HxWx1 -> HxWx3
+ * scn_convert_color_code: the code of an OpenCV name, SCN_E_UNSUPPORTED for any other name.
+ * scn_convert_color_name: the name of a code, NULL past the last one.
+ * scn_convert_color_channels: a code's input and output channel counts.
+ * scn_convert_color_u8: n dense frames of the code's input channels -> n dense frames of its output
+ *   channels, any alignment.  Pointer list; batches over 64 frames are split into launches.
+ * scn_convert_color_nv12: n NV12 surfaces (as scn_nv12_to_rgb24 takes them) converted to RGB24 with the
+ *   reference's arithmetic and then by `code`, without writing the RGB24 frame; identical to
+ *   scn_nv12_to_rgb24 followed by scn_convert_color_u8.  GRAY2* codes are SCN_E_BADARG here.
+ */
+SCN_API int scn_convert_color_code(const char* name);
+SCN_API const char* scn_convert_color_name(int code);
+SCN_API int scn_convert_color_channels(int code, int* in_channels, int* out_channels);
+SCN_API int scn_convert_color_u8(const uint8_t* const* host_src_ptrs, int n, int width, int height, int code,
+                                 uint8_t* const* host_dst_ptrs, void* stream);
+SCN_API int scn_convert_color_nv12(const uint8_t* const* host_luma_ptrs, const uint8_t* const* host_chroma_ptrs,
+                                   size_t pitch, int n, int width, int height, int code,
+                                   uint8_t* const* host_dst_ptrs, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * OpticalFlow  (replaces OpticalFlowKernelCPU::execute, tests/test_ops.cpp:79-98:
  *   cvtColor(COLOR_BGR2GRAY) on each RGB frame of the {0,1} stencil window, then
  *   cv::FarnebackOpticalFlow(numLevels, pyrScale, fastPyramids=false, winSize, numIters, polyN,

@@ -873,6 +873,7 @@ class Client:
                                                           "stdlib_args.proto")).read())
             self._op_protos["Blur"] = {"init": std["BlurArgs"]}
             self._op_protos["Resize"] = {"stream": std["ResizeArgs"]}
+            self._op_protos["ConvertColor"] = {"stream": std["ConvertColorArgs"]}
             self._op_protos["ImageEncoder"] = {"init": std["ImageEncoderArgs"]}
 
     # ---- table catalogue (reference client.py: ingest_videos :1009-1078, has_table, delete_table)

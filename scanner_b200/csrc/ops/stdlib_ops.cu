@@ -166,6 +166,87 @@ REGISTER_KERNEL(Resize, ResizeKernelGPU)
     .input_layout("frame", FrameLayout::NV12);
 
 // ---------------------------------------------------------------------------------------------
+// ConvertColor: scannertools' op (cv::cvtColor with ConvertColorArgs.conversion, a per-stream OpenCV code name),
+// bit-exact for the codes scn_convert_color_code knows.  Gray output is (H, W, 1).  A decoded NV12 element is
+// converted from the RGB24 frame the decoder would have delivered, without writing that frame.
+class ConvertColorKernelGPU : public BatchedKernel {
+ public:
+  ConvertColorKernelGPU(const KernelConfig& config) : BatchedKernel(config), device_(config.devices[0]) {}
+
+  void new_stream(const std::vector<u8>& args) override {
+    ConvertColorArgs a;
+    code_ = -1;
+    if (!a.ParseFromArray(args.data(), (int)args.size())) {
+      report_kernel_error("Could not parse ConvertColorArgs");
+      return;
+    }
+    code_ = scn_convert_color_code(a.conversion().c_str());
+    if (code_ < 0) {
+      std::string supported;
+      for (int c = 0; scn_convert_color_name(c); ++c) supported += std::string(c ? ", " : "") + scn_convert_color_name(c);
+      report_kernel_error("ConvertColor: unsupported conversion '" + a.conversion() + "'; supported: " + supported);
+      return;
+    }
+    SCN_CHECK(scn_convert_color_channels(code_, &in_channels_, &out_channels_));
+  }
+
+  void execute(const BatchedElements& input_columns, BatchedElements& output_columns) override {
+    const Elements& frames = input_columns[0];
+    if (frames.empty()) return;
+    CU_CHECK(cudaSetDevice(device_.id));
+    for_each_run(frames, [&](size_t i0, size_t i1, const Frame* f0) {
+      const i32 n = (i32)(i1 - i0);
+      // an NV12 element is a 1-channel frame too: its picture has three channels
+      const bool nv12 = is_nv12(f0);
+      const int channels = nv12 ? 3 : f0->channels();
+      std::string why;
+      if ((proto::FrameType)f0->type != proto::U8)
+        why = "expects uint8 frames, got type " + std::to_string((int)(proto::FrameType)f0->type);
+      else if (nv12 && (f0->channels() != 1 || f0->height() % 3 != 0 || (f0->width() & 1)))
+        why = "malformed NV12 frame element " + std::to_string(f0->height()) + "x" + std::to_string(f0->width());
+      else if (channels != in_channels_)
+        why = std::string(scn_convert_color_name(code_)) + " takes " + std::to_string(in_channels_) +
+              "-channel frames, got " + std::to_string(channels) + " channels";
+      if (!why.empty()) {
+        report_kernel_error("ConvertColor, row " + std::to_string(frames[i0].index) + ": " + why);
+        for (i32 i = 0; i < n; ++i) output_columns[0].push_back(Element());
+        return;
+      }
+      const int w = pic_width(f0), h = pic_height(f0);
+      std::vector<Frame*> outs = new_frames(device_, FrameInfo(h, w, out_channels_, FrameType::U8), n);
+      std::vector<const u8*> src;
+      std::vector<u8*> dst;
+      for (i32 i = 0; i < n; ++i) {
+        src.push_back(frames[i0 + i].as_const_frame()->data);
+        dst.push_back(outs[i]->data);
+      }
+      if (nv12) {
+        std::vector<const u8*> chroma;
+        for (const u8* p : src) chroma.push_back(p + (size_t)w * h);
+        SCN_CHECK(scn_convert_color_nv12(src.data(), chroma.data(), (size_t)w, n, w, h, code_, dst.data(),
+                                         device_stream(device_)));
+      } else {
+        SCN_CHECK(scn_convert_color_u8(src.data(), n, w, h, code_, dst.data(), device_stream(device_)));
+      }
+      for (i32 i = 0; i < n; ++i) insert_frame(output_columns[0], outs[i]);
+    });
+  }
+
+ private:
+  DeviceHandle device_;
+  int code_ = -1;
+  int in_channels_ = 0, out_channels_ = 0;
+};
+
+REGISTER_OP(ConvertColor).frame_input("frame").frame_output("frame").stream_protobuf_name("ConvertColorArgs");
+
+REGISTER_KERNEL(ConvertColor, ConvertColorKernelGPU)
+    .device(DeviceType::GPU)
+    .batch(64)
+    .num_devices(1)
+    .input_layout("frame", FrameLayout::NV12);
+
+// ---------------------------------------------------------------------------------------------
 class BlurKernelGPU : public BatchedKernel {
  public:
   BlurKernelGPU(const KernelConfig& config) : BatchedKernel(config), device_(config.devices[0]) {

@@ -154,6 +154,71 @@ def nv12_hist_resize(surfaces, width, height, dst_w, dst_h, plan=None, want_resi
     return hist, res
 
 
+def convert_color_code(name):
+    """OpenCV conversion name ('COLOR_RGB2GRAY', ...) -> (code, input channels, output channels)."""
+    L = cabi.lib()
+    code = L.scn_convert_color_code(name.encode())
+    if code < 0:
+        supported = []
+        while L.scn_convert_color_name(len(supported)):
+            supported.append(L.scn_convert_color_name(len(supported)).decode())
+        raise cabi.ScnError(f"unsupported conversion {name!r}; supported: {', '.join(supported)}")
+    cin, cout = ctypes.c_int(), ctypes.c_int()
+    cabi.check(L.scn_convert_color_channels(code, ctypes.byref(cin), ctypes.byref(cout)), "scn_convert_color_channels")
+    return code, cin.value, cout.value
+
+
+def convert_color(frames, code, width=None, height=None):
+    """cv2.cvtColor(frame, cv2.<code>) on the GPU, bit-exact.  `code` is the OpenCV name, e.g. 'COLOR_RGB2GRAY'.
+
+    frames: (N,H,W,C) uint8 CUDA tensor -> (N,H,W,C_out); a list of (H,W,C) tensors, shapes may differ -> list
+    (one launch per run of equal shape); or, with width and height, (N, H*3/2, pitch) NV12 surfaces (as
+    nv12_to_rgb takes them) -> (N,H,W,C_out), converted from the RGB24 frame nv12_to_rgb would give."""
+    cc, cin, cout = convert_color_code(code)
+    L = cabi.lib()
+    if width is not None:
+        _need_cuda(frames)
+        surfaces = frames.contiguous()
+        n = surfaces.shape[0]
+        lum, chr_, pitch = _surface_ptrs(surfaces, height)
+        out = torch.empty((n, height, width, cout), dtype=torch.uint8, device=surfaces.device)
+        lp, k1 = cabi.ptr_array(lum)
+        cp, k2 = cabi.ptr_array(chr_)
+        op, k3 = cabi.ptr_array([out.data_ptr() + i * height * width * cout for i in range(n)])
+        cabi.check(L.scn_convert_color_nv12(lp, cp, pitch, n, width, height, cc, op, _stream()),
+                   "scn_convert_color_nv12")
+        return out
+    def run(src_ptrs, h, w, c, device):
+        """frames of one shape -> one (n,h,w,C_out) tensor; the frames need not be 16-byte aligned"""
+        if c != cin:
+            raise cabi.ScnError(f"{code} takes {cin}-channel frames, got {c} channels")
+        out = torch.empty((len(src_ptrs), h, w, cout), dtype=torch.uint8, device=device)
+        sp, k1 = cabi.ptr_array(src_ptrs)
+        dp, k2 = cabi.ptr_array([out.data_ptr() + i * h * w * cout for i in range(len(src_ptrs))])
+        cabi.check(L.scn_convert_color_u8(sp, len(src_ptrs), w, h, cc, dp, _stream()), "scn_convert_color_u8")
+        return out
+
+    if isinstance(frames, torch.Tensor):
+        _need_cuda(frames)
+        assert frames.dtype == torch.uint8 and frames.dim() == 4
+        frames = frames.contiguous()
+        n, h, w, c = frames.shape
+        return run([frames.data_ptr() + i * h * w * c for i in range(n)], h, w, c, frames.device)
+    lst = [t.contiguous() for t in frames]
+    _need_cuda(*lst)
+    for t in lst:
+        assert t.dtype == torch.uint8 and t.dim() == 3
+    outs = []
+    i = 0
+    while i < len(lst):
+        j = i + 1
+        while j < len(lst) and lst[j].shape == lst[i].shape:
+            j += 1
+        outs += list(run([t.data_ptr() for t in lst[i:j]], *lst[i].shape, lst[i].device))
+        i = j
+    return outs
+
+
 def optical_flow_sequence(frames, workspace=None, pairs_per_call=None):
     """Flow of every consecutive pair of a clip: (N,H,W,3) uint8 -> (N-1,H,W,2) float32.  Every frame is expanded
     once (scn_farneback_u8c3_chain); pairs_per_call splits the clip over several calls on one workspace, the way
