@@ -7,7 +7,7 @@ import ctypes
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# SCN_KERNELS_LIB: developer switch used by tools/sweep_stream.py to time build variants of the library
+# SCN_KERNELS_LIB: developer switch to load another build of the library (to time two builds side by side)
 LIB_PATH = os.environ.get("SCN_KERNELS_LIB") or os.path.join(_HERE, "lib", "libscn_kernels.so")
 
 _c = ctypes

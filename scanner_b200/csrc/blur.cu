@@ -4,19 +4,16 @@
 // reference never writes the border of its freshly allocated frame -- here it is written as 0.
 // Integer, bit-exact on the interior.
 //
-//   box3_kernel   kernel_size 3 (BASELINE configs[2]).  A thread owns one 32-bit column of the byte
+// The launcher takes the first kernel that fits the batch:
+//   box_packed_kernel<K> kernel_size 2..31 on 16-byte aligned rows (every BASELINE frame size): u16x2 lanes, running
+//                 vertical sums, 128-bit loads two rows ahead; 3.9 TB/s at K = 3 (60 % of the copy peak), > 3 TB/s to K = 9.
+//   box3_kernel   kernel_size 3 on 4-byte aligned rows.  A thread owns one 32-bit column of the byte
 //                 image (4 bytes = 1 1/3 pixels) and walks down a strip of rows.  The three taps of
 //                 the horizontal pass are byte-shifted views of three neighbouring words (funnel
 //                 shifts), summed as packed u16x2 lanes; the vertical pass is a 3-row sliding sum
 //                 held in registers; /9 is an exact multiply-shift; four results are stored as one
 //                 32-bit word.  No shared memory: neighbouring threads' loads overlap in L1.
-//   box_packed_kernel<K> kernel_size 2..31 on 16-byte aligned rows (every BASELINE frame size): u16x2 lanes, running
-//                 vertical sums, 128-bit loads two rows ahead; 3.9 TB/s at K = 3 (60 % of the copy peak), > 3 TB/s to K = 9.
-//   box_stream_kernel    SCN_BLUR_PATH=stream only (r02 first kernel): bulk-async (cp.async.bulk + mbarrier) row
-//                 ring, sliding horizontal sums, running vertical sums: O(1) work per sample.
 //   box_generic_kernel   the rest (unaligned or tiny frames, kernel_size 1): shared-memory tile, direct sums.
-#include <string.h>
-
 #include "scn_common.cuh"
 
 namespace scn {
@@ -167,165 +164,6 @@ box_generic_kernel(PtrBatch src, MutPtrBatch dst, int width, int height, int fl,
 }
 
 // ---------------------------------------------------------------------------------------------
-// box_stream_kernel: any kernel_size, O(1) work per sample.  A CTA owns a strip of kStripBytes byte
-// columns and walks down kStripRows output rows:
-//   * each input row segment arrives by ONE bulk-async copy (cp.async.bulk global -> shared, completion on
-//     an mbarrier) into a ring of kRowSlots slots, issued kRowSlots - 1 rows ahead by one thread;
-//   * horizontal pass: a thread owns 4 pixels (12 bytes); the first pixel's window is summed directly, the
-//     next three slide (add the entering sample, drop the leaving one);
-//   * vertical pass: running column sums in registers: + this row's horizontal sums, - those of the row
-//     that leaves the window (kept in a shared-memory ring of k rows of u16);
-//   * out = sum / k^2 by an exact multiply-shift, 12 bytes stored per thread (a warp writes 384 contiguous
-//     bytes).  Border samples (window not inside the frame) are written as 0, so whatever a row segment
-//     holds beyond the frame never reaches an output.
-// Needs 16-byte aligned rows (width % 16 == 0, 16-byte aligned frames).
-constexpr int kStripBytes = 3072;  // 1024 pixels: 256 threads x 12 bytes
-constexpr int kStripRows = 128;
-constexpr int kRowSlots = 4;
-constexpr int BS = 256;
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n.reg .pred p;\nWAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\nbra WAIT_%=;\nDONE_%=:\n}" ::"r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-               "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
-}
-
-__global__ void __launch_bounds__(BS)
-box_stream_kernel(PtrBatch src, MutPtrBatch dst, int width, int height, int fl, int fr, uint32_t div_magic) {
-  extern __shared__ __align__(128) uint8_t smem_raw[];
-  __shared__ __align__(8) unsigned long long bars[kRowSlots];
-  const int k = fl + fr + 1;
-  const int row_bytes = width * 3;
-  const int x0b = blockIdx.x * kStripBytes;                       // first output byte column of the strip
-  const int out_wb = min(kStripBytes, row_bytes - x0b);
-  // bytes of a row this strip reads: [c0, c1), widened to 16-byte boundaries, clipped to the row
-  const int c0 = max(0, (x0b - 3 * fl) & ~15);
-  const int c1 = min(row_bytes, (x0b + out_wb + 3 * fr + 15) & ~15);
-  const int seg = c1 - c0;
-  const int lead = x0b - c0;                                      // strip byte 0 sits at segment byte `lead`
-  // a slot: kLeftPad bytes nobody writes (reads of a border pixel's window may fall before the segment),
-  // then the segment: at most kStripBytes + 2 * (45 + 15) bytes (KMAX = 31: fl, fr <= 15)
-  constexpr int kLeftPad = 48;
-  constexpr int kSegMax = kLeftPad + kStripBytes + 128;
-  uint8_t* rows = smem_raw;                                       // kRowSlots x kSegMax
-  uint16_t* hring = reinterpret_cast<uint16_t*>(smem_raw + kRowSlots * kSegMax);  // k x kStripBytes
-  const uint8_t* __restrict__ s = src.p[blockIdx.z];
-  uint8_t* __restrict__ d = dst.p[blockIdx.z];
-  const int y_out0 = blockIdx.y * kStripRows, y_out1 = min(height, y_out0 + kStripRows);
-  // input rows needed: [y_out0 - fl, y_out1 + fr), clipped; rows outside the frame only feed border outputs
-  const int r_first = max(0, y_out0 - fl), r_last = min(height, y_out1 + fr);
-  const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(bars);
-  const uint32_t rows_s = (uint32_t)__cvta_generic_to_shared(rows);
-  const int t = threadIdx.x;
-  if (t == 0) {
-    for (int i = 0; i < kRowSlots; ++i) mbar_init(bar0 + 8 * i, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  auto issue = [&](int r) {  // thread 0: bulk copy of input row r into its slot
-    const int slot = (r - r_first) % kRowSlots;
-    mbar_expect_tx(bar0 + 8 * slot, (uint32_t)seg);
-    bulk_g2s(rows_s + slot * kSegMax + kLeftPad, s + (size_t)r * row_bytes + c0, (uint32_t)seg, bar0 + 8 * slot);
-  };
-  if (t == 0)
-    for (int r = r_first; r < min(r_last, r_first + kRowSlots - 1); ++r) issue(r);
-
-  const int b0 = 12 * t;                       // this thread's first output byte in the strip
-  const bool active = b0 < out_wb;             // out_wb is a multiple of 12 (row_bytes % 48 == 0, strips of 3072)
-  uint32_t vsum[12];
-#pragma unroll
-  for (int i = 0; i < 12; ++i) vsum[i] = 0;
-  // x-interior flags of the 4 pixels
-  bool xin[4];
-#pragma unroll
-  for (int p = 0; p < 4; ++p) {
-    const int px = (x0b + b0) / 3 + p;
-    xin[p] = px >= fl && px < width - fr;
-  }
-
-  for (int r = r_first; r < r_last; ++r) {
-    const int idx = r - r_first, slot = idx % kRowSlots;
-    if (t == 0 && r + kRowSlots - 1 < r_last) issue(r + kRowSlots - 1);   // its slot was released by the last barrier
-    mbar_wait(bar0 + 8 * slot, (uint32_t)((idx / kRowSlots) & 1));
-    uint16_t h[12];
-    if (active) {
-      const uint8_t* row = rows + slot * kSegMax + kLeftPad + lead + b0;
-      // window of pixel 0 summed directly: samples at byte offsets 3 * (j - fl) + ch (a border pixel's window
-      // may start in the pad or end in stale bytes: its output is masked); pixels 1..3 slide
-      uint32_t a0 = 0, a1 = 0, a2 = 0;
-      const int lo = -3 * fl;
-      for (int j = 0; j < k; ++j) {
-        a0 += row[lo + 3 * j + 0];
-        a1 += row[lo + 3 * j + 1];
-        a2 += row[lo + 3 * j + 2];
-      }
-      h[0] = (uint16_t)a0;
-      h[1] = (uint16_t)a1;
-      h[2] = (uint16_t)a2;
-#pragma unroll
-      for (int p = 1; p < 4; ++p) {
-        a0 += row[3 * (p + fr) + 0] - row[3 * (p - 1 - fl) + 0];
-        a1 += row[3 * (p + fr) + 1] - row[3 * (p - 1 - fl) + 1];
-        a2 += row[3 * (p + fr) + 2] - row[3 * (p - 1 - fl) + 2];
-        h[3 * p + 0] = (uint16_t)a0;
-        h[3 * p + 1] = (uint16_t)a1;
-        h[3 * p + 2] = (uint16_t)a2;
-      }
-      // vertical running sums: + this row, - the row leaving the window (input row r - k, if it was fed);
-      // the ring holds 12 u16 per thread = three 8-byte words
-      uint2* hslot = reinterpret_cast<uint2*>(hring + (size_t)(idx % k) * kStripBytes + b0);
-      if (idx >= k) {
-#pragma unroll
-        for (int q = 0; q < 3; ++q) {
-          const uint2 o = hslot[q];
-          vsum[4 * q + 0] -= o.x & 0xFFFFu;
-          vsum[4 * q + 1] -= o.x >> 16;
-          vsum[4 * q + 2] -= o.y & 0xFFFFu;
-          vsum[4 * q + 3] -= o.y >> 16;
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 12; ++i) vsum[i] += h[i];
-#pragma unroll
-      for (int q = 0; q < 3; ++q)
-        hslot[q] = make_uint2((uint32_t)h[4 * q] | ((uint32_t)h[4 * q + 1] << 16), (uint32_t)h[4 * q + 2] | ((uint32_t)h[4 * q + 3] << 16));
-      // output row y = r - fr is complete once input row r is in (its window is rows y-fl .. y+fr)
-      const int y = r - fr;
-      if (y >= y_out0 && y < y_out1) {
-        const bool yin = y >= fl && y < height - fr;
-        uint32_t o[12];
-#pragma unroll
-        for (int i = 0; i < 12; ++i) o[i] = (yin && xin[i / 3]) ? __umulhi(vsum[i], div_magic) : 0u;
-        uint32_t* dp = reinterpret_cast<uint32_t*>(d + (size_t)y * row_bytes + x0b + b0);
-        dp[0] = o[0] | (o[1] << 8) | (o[2] << 16) | (o[3] << 24);
-        dp[1] = o[4] | (o[5] << 8) | (o[6] << 16) | (o[7] << 24);
-        dp[2] = o[8] | (o[9] << 8) | (o[10] << 16) | (o[11] << 24);
-      }
-    }
-    __syncthreads();  // everyone is done with this row's slot: thread 0 may refill it next iteration
-  }
-  // output rows whose window reaches below the frame are border rows: written as 0 (their input rows never came)
-  for (int y = max(y_out0, r_last - fr); y < y_out1; ++y) {
-    if (active && y >= 0) {
-      uint32_t* dp = reinterpret_cast<uint32_t*>(d + (size_t)y * row_bytes + x0b + b0);
-      dp[0] = dp[1] = dp[2] = 0u;
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
 // box_packed_kernel<K>: kernel_size 2..31 on 16-byte aligned rows, all arithmetic on packed u16x2 lanes.
 //   * a thread owns one 16-byte column (a "quad": 4 words) and walks down a strip of rows; a warp owns 32
 //     neighbouring quads of which the R on each side are halo (R = 1 for K <= 11, 2 up to K = 21, else 3);
@@ -341,7 +179,7 @@ box_stream_kernel(PtrBatch src, MutPtrBatch dst, int width, int height, int fl, 
 //     compile-time constant.  Lane sums stay below 255 K^2 <= 65280 for K <= 16; above, the terms are summed in
 //     groups of 8 (8 x 255 x 31 fits a lane) and the groups unpacked into 32-bit sums;
 //   * out = sum / K^2 by the exact multiply-shift, border samples masked to 0, one 128-bit store per thread.
-// ~6-12 instructions per byte (K = 3..15) where box_stream_kernel spends 15 and more on byte loads.
+// ~6-12 instructions per byte (K = 3..15).
 constexpr int BP_WARPS = 4;
 template <int K>
 struct PackedGeom {
@@ -513,19 +351,9 @@ int launch_blur(const uint8_t* const* sp, int n, int width, int height, int ksiz
     bool aligned16 = (width % 16) == 0 && height >= k;
     for (int i = 0; i < cnt; ++i)
       if (((uintptr_t)s.p[i] | (uintptr_t)d.p[i]) & 15) aligned16 = false;
-    static const bool stream3 = [] {
-      const char* e = getenv("SCN_BLUR3");
-      return e && e[0] == 's';  // SCN_BLUR3=stream: kernel_size 3 through the streaming kernel too (measurement switch)
-    }();
-    // SCN_BLUR_PATH=stream keeps kernel sizes 2..16 on the byte-wise streaming kernel; =box3 keeps kernel_size 3 on
-    // box3_kernel even when the rows are 16-byte aligned (measurement switches)
-    static const int path = [] {
-      const char* e = getenv("SCN_BLUR_PATH");
-      return !e ? 0 : strcmp(e, "stream") == 0 ? 1 : strcmp(e, "box3") == 0 ? 2 : 0;
-    }();
-    if (aligned16 && k >= 2 && k <= 31 && path != 1 && (ksize != 3 || path != 2)) {
+    if (aligned16 && k >= 2) {
       const unsigned d2 = (unsigned)(k * k);
-      const uint32_t magic = (uint32_t)((1ull << 32) / d2) + 1u;
+      const uint32_t magic = (uint32_t)((1ull << 32) / d2) + 1u;  // floor(v * magic / 2^32) == v / d2 for v <= 255 * d2
       const int quads = width * 3 / 16;
       const int out_quads = 32 - 2 * ((3 * fr + 15) / 16);
       const unsigned gx = (unsigned)((quads + out_quads * BP_WARPS - 1) / (out_quads * BP_WARPS));
@@ -544,20 +372,6 @@ int launch_blur(const uint8_t* const* sp, int n, int width, int height, int ksiz
         SCN_BP_CASE(29) SCN_BP_CASE(30) SCN_BP_CASE(31)
 #undef SCN_BP_CASE
       }
-    } else if (aligned16 && k >= 2 && (ksize != 3 || stream3)) {
-      const size_t smem_s = (size_t)kRowSlots * (48 + kStripBytes + 128) + (size_t)k * kStripBytes * 2;
-      static bool attr2 = false;
-      if (!attr2) {
-        cudaError_t e = cudaFuncSetAttribute(box_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 210 * 1024);
-        if (e != cudaSuccess) return (int)e;
-        attr2 = true;
-      }
-      const unsigned d2 = (unsigned)(k * k);
-      const uint32_t magic = (uint32_t)((1ull << 32) / d2) + 1u;  // floor(v * magic / 2^32) == v / d2 for v <= 255 * d2
-      dim3 grid((unsigned)((width * 3 + kStripBytes - 1) / kStripBytes), (unsigned)((height + kStripRows - 1) / kStripRows),
-                (unsigned)cnt);
-      LaunchScope ls("box_stream_kernel", st);
-      box_stream_kernel<<<grid, BS, smem_s, st>>>(s, d, width, height, fl, fr, magic);
     } else if (ksize == 3 && aligned) {
       const int wpr = width * 3 / 4;
       dim3 grid((unsigned)((wpr + B3_THREADS - 1) / B3_THREADS), (unsigned)((height + B3_ROWS - 1) / B3_ROWS),

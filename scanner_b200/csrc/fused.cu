@@ -6,19 +6,11 @@
 // destination pixel.  Results are bit-identical to the three-pass composition.
 #include "nv12_stream.cuh"
 
-#ifndef SCN_NV12_RESIZE_DEFAULT
-#define SCN_NV12_RESIZE_DEFAULT kOverlap
-#endif
 #include "nv12_math.cuh"
+#include "resize_plan.cuh"
 #include "scn_common.cuh"
 
 namespace scn {
-
-struct Tap {
-  int32_t i0, i1, w0, w1;
-};
-constexpr size_t kPlanHeaderBytes = 32;
-
 namespace {
 
 constexpr int HT = 256;
@@ -106,11 +98,11 @@ nv12_resize_kernel(PtrBatch lumas, PtrBatch chromas, size_t pitch, int width, in
     o[2] = (uint8_t)((a.b + b.b + c.b + d.b + 2) >> 2);
     return;
   }
-  // Instruction-bound: four exact NV12 -> RGB conversions per destination pixel.  Two leaner-looking forms were measured and were not faster: the XU-converting tap chain of
-  // nv12_stream.cuh (46 us instead of 37 us per 64 frames) and a row-organised kernel (a CTA per destination row,
-  // uniform row addresses, u16 chroma loads, chroma terms computed once per sample, mulhi blend: 312 static
-  // instructions, the same 37 us).
-  const Tap* __restrict__ xt = reinterpret_cast<const Tap*>(plan + kPlanHeaderBytes);
+  // Instruction-bound: four exact NV12 -> RGB conversions per destination pixel.  Two leaner-looking forms were
+  // measured and were not faster: a tap chain converting bytes to float on the XU pipe (46 us instead of 37 us per
+  // 64 frames) and a row-organised kernel (a CTA per destination row, uniform row addresses, u16 chroma loads, chroma
+  // terms computed once per sample, mulhi blend: 312 static instructions, the same 37 us).
+  const Tap* __restrict__ xt = reinterpret_cast<const Tap*>(plan + sizeof(PlanHeader));
   const Tap* __restrict__ yt = xt + dw;
   const int4 tx = __ldg(reinterpret_cast<const int4*>(xt + dx));
   const int4 ty = __ldg(reinterpret_cast<const int4*>(yt + dy));
@@ -192,34 +184,18 @@ extern "C" int scn_nv12_hist_resize(const uint8_t* const* host_luma_ptrs,
     if (e != cudaSuccess) return (int)e;
   }
   const int quads = (width + 3) / 4;
-  // Large aligned surfaces take the one-pass streaming kernel (nv12_stream.cuh): histogram and, when
-  // both are wanted, the Resize rows of every span right behind it.  Everything else (tiny, ragged or
-  // unaligned surfaces; Resize alone) runs the generic kernels below.
+  // Large aligned surfaces take the streaming histogram kernel (nv12_stream.cuh); tiny, ragged or unaligned ones
+  // take nv12_hist_kernel.  Resize is nv12_resize_kernel either way.
   bool stream_ok = do_hist;
   for (int i0 = 0; i0 < n && stream_ok; i0 += SCN_MAX_PTRS) {
     const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
     stream_ok = nvs::eligible(host_luma_ptrs + i0, host_chroma_ptrs + i0, cnt, pitch, width, height);
   }
-  // How Histogram + Resize of the same surfaces run (SCN_NV12_RESIZE):
-  //   fused    the Resize rows are produced inside the streaming pass (one HBM read of the surface);
-  //   split    streaming histogram kernel, then nv12_resize_kernel behind it on the same stream;
-  //   overlap  nv12_resize_kernel on a side stream next to the streaming kernel.
-  enum { kFused, kSplit, kOverlap };
-  static const int resize_mode = [] {
-    const char* e = getenv("SCN_NV12_RESIZE");
-    if (e && e[0] == 'f') return (int)kFused;
-    if (e && e[0] == 'o') return (int)kOverlap;
-    if (e && e[0] == 's') return (int)kSplit;
-    return (int)SCN_NV12_RESIZE_DEFAULT;
-  }();
-  // (the exact-2x Resize, an INTER_AREA average, is not produced inside the streaming pass)
-  if (stream_ok && !(do_resize && (resize_mode != kFused || area2x)))
-    return nvs::launch(host_luma_ptrs, host_chroma_ptrs, n, pitch, width, height, hist_out, do_resize ? host_dst_ptrs : nullptr,
-                       (do_resize && !area2x) ? (const uint8_t*)plan + kPlanHeaderBytes : nullptr, dst_w, dst_h, area2x ? 1 : 0, st);
+  // Histogram and Resize together: the Resize kernels go to the side stream (see SideStream), forked before any
+  // histogram kernel is enqueued so that both can be resident together
   SideStream* side = nullptr;
   cudaStream_t rst = st;
-  if (stream_ok && do_resize && resize_mode == kOverlap && (side = side_stream()) != nullptr) {
-    // fork before the histogram kernel is enqueued so both kernels can be resident together
+  if (do_hist && do_resize && (side = side_stream()) != nullptr) {
     if (cudaEventRecord(side->fork, st) != cudaSuccess || cudaStreamWaitEvent(side->stream, side->fork, 0) != cudaSuccess) {
       cudaGetLastError();
       side = nullptr;
@@ -227,22 +203,9 @@ extern "C" int scn_nv12_hist_resize(const uint8_t* const* host_luma_ptrs,
       rst = side->stream;
     }
   }
-  if (stream_ok) {
-    const int rc0 = nvs::launch(host_luma_ptrs, host_chroma_ptrs, n, pitch, width, height, hist_out, nullptr, nullptr, 0, 0, 0, st);
-    if (rc0) return rc0;
-  }
-  const bool hist_done = stream_ok;
-  // generic path: the resize kernels of this call go to the side stream (see SideStream)
-  if (!hist_done && do_hist && do_resize && (side = side_stream()) != nullptr) {
-    if (cudaEventRecord(side->fork, st) != cudaSuccess || cudaStreamWaitEvent(side->stream, side->fork, 0) != cudaSuccess) {
-      cudaGetLastError();
-      side = nullptr;
-    } else {
-      rst = side->stream;
-    }
-  }
-  int rc = 0;
-  for (int i0 = 0; i0 < n && rc == 0; i0 += SCN_MAX_PTRS) {
+  int rc = stream_ok ? nvs::launch(host_luma_ptrs, host_chroma_ptrs, n, pitch, width, height, hist_out, st) : 0;
+  // the generic histogram and the Resize, per chunk of 64 surfaces
+  for (int i0 = 0; i0 < n && rc == 0 && (do_resize || !stream_ok); i0 += SCN_MAX_PTRS) {
     const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
     PtrBatch l, c;
     MutPtrBatch d;
@@ -253,7 +216,7 @@ extern "C" int scn_nv12_hist_resize(const uint8_t* const* host_luma_ptrs,
       d.p[i] = do_resize ? host_dst_ptrs[i0 + i] : nullptr;
       if (((uintptr_t)l.p[i] | (uintptr_t)c.p[i]) & 3) vec_ok = 0;
     }
-    if (do_hist && !hist_done) {
+    if (do_hist && !stream_ok) {
       const int gx = (quads + HT - 1) / HT;
       int gy = (sm_count() * 8 + gx * cnt - 1) / (gx * cnt);
       if (gy < 1) gy = 1;

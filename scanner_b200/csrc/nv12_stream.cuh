@@ -1,7 +1,7 @@
-// nv12_stream.cuh -- ONE pass over NV12 decoder surfaces for BASELINE configs[1]:
-//     NV12 -> RGB -> { Histogram (tests/test_ops.cpp:19-49), Resize (tests/test_ops.cpp:124-162) }
+// nv12_stream.cuh -- ONE pass over NV12 decoder surfaces for the Histogram of BASELINE configs[1]:
+//     NV12 -> RGB -> Histogram (tests/test_ops.cpp:19-49)
 // with the reference's NV12->RGB arithmetic (scanner/util/image.cu:67-200 as nvcc contracts it, see
-// nv12_math.cuh) and neither the RGB frame nor a second read of the surface in HBM.
+// nv12_math.cuh) and no RGB frame in HBM.
 //
 // Design (the kernel is bound by instruction issue, not by HBM: every choice below trades ALU, FMA and
 // XU (conversion) pipe work against each other so that no pipe is the only busy one):
@@ -21,10 +21,8 @@
 //             x = fma.sat(cr, k2, gi), m = floor(32 x) in 0..31, upper clamp by a second .sat;
 //   * floor: fma.rm(x, k, 2^23) leaves the integer in the mantissa; four bins are packed into the
 //     16-bit selector of a PRMT with IMADs on the float's bits (R, B) / an FMA accumulate (G);
-//   * counting: PRMT as an 8-entry one-hot LUT + bit-sliced carry-save adders (csa_core.cuh);
-//   * Resize: when a warp has finished the histogram of a span of rows it produces the destination
-//     rows whose first tap row starts in that span -- the taps were streamed moments ago and come
-//     from L1/L2, so the surface crosses HBM once.
+//   * counting: PRMT as an 8-entry one-hot LUT + bit-sliced carry-save adders (csa_core.cuh).
+// Resize of the same surfaces is nv12_resize_kernel (fused.cu), run beside this kernel on a side stream.
 #pragma once
 #include "csa_core.cuh"
 #include "nv12_math.cuh"
@@ -33,23 +31,13 @@
 namespace scn {
 namespace nvs {
 
-#ifndef NVS_WARPS
-#define NVS_WARPS 12
-#endif
-#ifndef NVS_STAGES
-#define NVS_STAGES 4
-#endif
-#ifndef NVS_CHROMA_XU
-#define NVS_CHROMA_XU 0   // 1: chroma bytes -> float on the XU pipe too (64 conversions per step)
-#endif
-constexpr int kWarps = NVS_WARPS;
+constexpr int kWarps = 12;
 constexpr int kThreads = kWarps * 32;
-constexpr int kStages = NVS_STAGES;
+constexpr int kStages = 4;
 static_assert((kStages & (kStages - 1)) == 0, "the ring index is a mask");
 constexpr int kPlanes = 10;
 constexpr int kHi = kPlanes - 3;   // planes 3..9
 constexpr int kMaxSteps = 127;     // 127 * 8 words per accumulator <= 1023
-constexpr int kResizeChunk = 16;   // steps between Resize calls (power of two)
 constexpr size_t kSmemBytes = (size_t)kWarps * kStages * 4 * 32 * 16;
 
 using Acc = csa::Acc8<kHi>;
@@ -113,15 +101,6 @@ struct Chroma2 {
 };
 __device__ __forceinline__ Chroma2 chroma_terms(uint32_t cw) {
   Chroma2 c;
-#if NVS_CHROMA_XU
-  // XU pipe: plain floats; (cf - 128) * k is computed exactly inside one FMA (128 * k is a
-  // power-of-two multiple of k, so the addend is exact)
-  const f2 cb = pack2(byte_f<0>(cw), byte_f<2>(cw)), cr = pack2(byte_f<1>(cw), byte_f<3>(cw));
-  c.tb = fma2(cb, splat(kBC), splat(-128.0f * kBC));
-  c.cr = fma2(cr, splat(kRC), splat(-128.0f * kRC));
-  c.tg = fma2(cb, splat(kKG1), splat(-128.0f * kKG1));
-  c.crc = add2(cr, splat(-128.0f));
-#else
   // ALU pipe: PRMT builds the bits of 2^23 + byte; one exact FADD removes the bias and centres
   const f2 cbc = add2(pack2(__uint_as_float(prmt(cw, 0x4B000000u, 0x7440u)), __uint_as_float(prmt(cw, 0x4B000000u, 0x7442u))),
                       splat(-(kMagic + 128.0f)));
@@ -130,7 +109,6 @@ __device__ __forceinline__ Chroma2 chroma_terms(uint32_t cw) {
   c.tb = mul2(cbc, splat(kBC));
   c.cr = mul2(c.crc, splat(kRC));
   c.tg = mul2(cbc, splat(kKG1));
-#endif
   return c;
 }
 
@@ -206,10 +184,6 @@ __device__ const uint32_t g_lut_lo[32] = {
     csa::kLutLo, csa::kLutLo, csa::kLutLo, csa::kLutLo, csa::kLutLo, csa::kLutLo, csa::kLutLo, csa::kLutLo,
     csa::kLutLo, csa::kLutLo, csa::kLutLo, csa::kLutLo, csa::kLutLo, csa::kLutLo, csa::kLutLo, csa::kLutLo};
 
-struct Tap {
-  int32_t i0, i1, w0, w1;
-};
-
 struct Params {
   PtrBatch luma, chroma;
   size_t pitch;
@@ -219,10 +193,6 @@ struct Params {
   uint32_t units_per_frame;   // units_per_row * height / 2
   uint32_t steps_per_frame;   // ceil(units_per_frame / 32)
   uint64_t total_steps;
-  // Resize (all zero when only the histogram is wanted)
-  MutPtrBatch dst;
-  const Tap* xt;              // dw column taps, then dh row taps
-  int dw, dh, area2x;
 };
 
 __device__ __forceinline__ uint32_t lane_count(const Acc& a, int lane) {
@@ -250,112 +220,6 @@ __device__ __forceinline__ uint4 lds128(uint32_t smem_addr) {
   return r;
 }
 
-// ---- Resize taps for the destination rows a chunk of steps owns ---------------------------------
-// OpenCV INTER_LINEAR u8 (11-bit fixed point) on RGB values converted from the four tapped NV12
-// pixels; the exact-2x case is the INTER_AREA average (tests/test_ops.cpp:156, oracle orc_resize_*).
-struct ResizeArgs {   // by value: a non-inlined function cannot address the kernel parameter block
-  const uint8_t* luma;
-  const uint8_t* chroma;
-  uint8_t* dst;
-  const Tap* xt;
-  size_t pitch;
-  int height, dw, dh;
-  uint32_t units_per_row;
-};
-
-// Everything about one tapped source row that does not depend on the column: where its luma and chroma bytes
-// start and whether its chroma is the rounded average with the next chroma row (odd luma rows, image.cu:133-151)
-struct TapRow {
-  const uint8_t* luma;
-  const uint8_t* chroma;
-  size_t next;   // 0: no averaging, else the distance to the second chroma row
-};
-__device__ __forceinline__ TapRow tap_row(const ResizeArgs& a, int y) {
-  const int yc = y >> 1;
-  TapRow r;
-  r.luma = a.luma + (size_t)y * a.pitch;
-  r.chroma = a.chroma + (size_t)yc * a.pitch;
-  r.next = ((y & 1) && yc < (a.height >> 1) - 1) ? a.pitch : 0;
-  return r;
-}
-
-// One tapped pixel -> 8-bit RGB, the exact chain (nv12_math.cuh) with byte -> float on the XU pipe.
-__device__ __forceinline__ Rgb8 tap_rgb(const TapRow& row, int x) {
-  const uint8_t* cp = row.chroma + (x & ~1);
-  uint32_t c = __ldg(reinterpret_cast<const uint16_t*>(cp));                 // Cb | Cr << 8 (2-byte aligned)
-  if (row.next) {
-    const uint32_t c2 = __ldg(reinterpret_cast<const uint16_t*>(cp + row.next));
-    c = (c | c2) - (((c ^ c2) & 0xFEFEu) >> 1);                              // per byte (a + b + 1) >> 1
-  }
-  const float yf = (float)__ldg(row.luma + x);
-  const float cbc = byte_f<0>(c) - 128.0f, crc = byte_f<1>(c) - 128.0f;
-  constexpr float kKR = 4.0f * 1.596f * kS, kKB = 4.0f * 2.0172f * kS, kTop = 1023.0f * kS;
-  const float r = fma_sat(crc, kKR, __fmul_rn(yf, kCY));
-  const float g = fma_sat(crc, kKG2, __fmaf_rn(yf, kCY, __fmul_rn(cbc, kKG1)));
-  const float b = fma_sat(yf, kCY, __fmul_rn(cbc, kKB));
-  auto u8 = [&](float v) {  // floor(512 * min(v, 1023/2048)) == ((unsigned)min(value, 1023)) >> 2
-    float q;
-    asm("fma.rm.f32 %0, %1, %2, %3;" : "=f"(q) : "f"(fminf(v, kTop)), "f"(512.0f), "f"(kMagic));
-    return __float_as_uint(q) & 0xFFu;
-  };
-  return Rgb8{u8(r), u8(g), u8(b)};
-}
-
-struct Rgb24 {
-  uint8_t r, g, b;
-};
-// one destination pixel of the row whose tap rows are r0 / r1 with weights b0 / b1 (the read-only loads of its
-// four taps come first: callers interleave several)
-__device__ __forceinline__ Rgb24 resize_pixel(const ResizeArgs& a, const TapRow& r0, const TapRow& r1, int b0, int b1, int dx) {
-  const int4 tx = __ldg(reinterpret_cast<const int4*>(a.xt + dx));
-  const Rgb8 p00 = tap_rgb(r0, tx.x), p01 = tap_rgb(r0, tx.y);
-  const Rgb8 p10 = tap_rgb(r1, tx.x), p11 = tap_rgb(r1, tx.y);
-  const int a0 = tx.z, a1 = tx.w;
-  auto blend = [&](uint32_t v00, uint32_t v01, uint32_t v10, uint32_t v11) {
-    const int h0 = (int)v00 * a0 + (int)v01 * a1, h1 = (int)v10 * a0 + (int)v11 * a1;
-    return (uint8_t)((((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2);
-  };
-  return Rgb24{blend(p00.r, p01.r, p10.r, p11.r), blend(p00.g, p01.g, p10.g, p11.g), blend(p00.b, p01.b, p10.b, p11.b)};
-}
-
-// Destination rows whose first tap row starts in units [u0, u1) of the frame (row-pair-major unit order).
-// Called every kResizeChunk steps from the streaming loop: the tapped rows were streamed moments ago (or
-// are about to be), so the gathers hit L1/L2 and the surface still crosses HBM once.  Not inlined: the
-// streaming loop keeps its registers (the call saves what it needs), this path runs once per chunk.
-// (The exact-2x case, OpenCV's INTER_AREA average, is left to nv12_resize_kernel: the launcher does not fuse it.)
-__device__ __noinline__ void resize_units(ResizeArgs a, uint32_t u0, uint32_t u1, int lane) {
-  const uint32_t p0 = (u0 + a.units_per_row - 1) / a.units_per_row;  // first row pair starting in the range
-  const uint32_t p1 = (u1 + a.units_per_row - 1) / a.units_per_row;  // first row pair starting after it
-  const int r0 = (int)(2 * p0), r1 = (int)(2 * p1);
-  if (r0 >= r1) return;
-  const Tap* yt = a.xt + a.dw;
-  // the row taps ascend: binary search for the first dy whose first tap row is >= r0
-  int lo = 0, hi = a.dh;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (__ldg(&yt[mid].i0) < r0) lo = mid + 1;
-    else hi = mid;
-  }
-  for (int dy = lo; dy < a.dh; ++dy) {
-    const int4 ty = __ldg(reinterpret_cast<const int4*>(yt + dy));
-    if (ty.x >= r1) break;
-    const TapRow t0 = tap_row(a, ty.x), t1 = tap_row(a, ty.y);
-    uint8_t* row = a.dst + (size_t)dy * a.dw * 3;
-    // two destination pixels per iteration: the gathers of both are in flight together
-    for (int dx = lane; dx < a.dw; dx += 64) {
-      const int dx2 = dx + 32 < a.dw ? dx + 32 : dx;
-      const Rgb24 p = resize_pixel(a, t0, t1, ty.z, ty.w, dx), q = resize_pixel(a, t0, t1, ty.z, ty.w, dx2);
-      row[dx * 3 + 0] = p.r;
-      row[dx * 3 + 1] = p.g;
-      row[dx * 3 + 2] = p.b;
-      row[dx2 * 3 + 0] = q.r;
-      row[dx2 * 3 + 1] = q.g;
-      row[dx2 * 3 + 2] = q.b;
-    }
-  }
-}
-
-template <bool kResize>
 static __global__ void __launch_bounds__(kThreads, 1)
 nv12_stream_kernel(const Params prm, int32_t* __restrict__ out) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -474,14 +338,6 @@ nv12_stream_kernel(const Params prm, int32_t* __restrict__ out) {
         fold_step(A[c], cA[c], (int)step);
         fold_step(B[c], cB[c], (int)step);
       }
-      if constexpr (kResize) {
-        if ((step & (kResizeChunk - 1)) == kResizeChunk - 1 || step + 1 == ns) {
-          const uint32_t c0s = step & ~(uint32_t)(kResizeChunk - 1);
-          const ResizeArgs ra{prm.luma.p[frame], prm.chroma.p[frame], prm.dst.p[frame], prm.xt, prm.pitch, prm.height,
-                              prm.dw, prm.dh, prm.units_per_row};
-          resize_units(ra, (s0 + c0s) * 32u, min((s0 + step + 1) * 32u, prm.units_per_frame), lane);
-        }
-      }
     }
 
     // ---- flush the span
@@ -531,14 +387,13 @@ inline bool eligible(const uint8_t* const* lp, const uint8_t* const* cp, int n, 
   return true;
 }
 
-// `out` must already be zeroed.  dst / plan / dw / dh describe the Resize (dst == nullptr: histogram only).
+// `out` must already be zeroed.
 inline int launch(const uint8_t* const* lp, const uint8_t* const* cp, int n, size_t pitch, int width, int height,
-                  int32_t* out, uint8_t* const* dst, const void* plan_taps, int dw, int dh, int area2x, cudaStream_t st) {
+                  int32_t* out, cudaStream_t st) {
   static std::atomic<int> attr_done{0};
   if (!attr_done.load(std::memory_order_acquire)) {
-    cudaError_t e1 = cudaFuncSetAttribute(nv12_stream_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    cudaError_t e2 = cudaFuncSetAttribute(nv12_stream_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e1 != cudaSuccess || e2 != cudaSuccess) return (int)(e1 != cudaSuccess ? e1 : e2);
+    const cudaError_t e = cudaFuncSetAttribute(nv12_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    if (e != cudaSuccess) return (int)e;
     attr_done.store(1, std::memory_order_release);
   }
   for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
@@ -547,7 +402,6 @@ inline int launch(const uint8_t* const* lp, const uint8_t* const* cp, int n, siz
     for (int i = 0; i < cnt; ++i) {
       p.luma.p[i] = lp[i0 + i];
       p.chroma.p[i] = cp[i0 + i];
-      p.dst.p[i] = dst ? dst[i0 + i] : nullptr;
     }
     p.pitch = pitch;
     p.width = width;
@@ -557,17 +411,12 @@ inline int launch(const uint8_t* const* lp, const uint8_t* const* cp, int n, siz
     p.units_per_frame = p.units_per_row * (uint32_t)(height / 2);
     p.steps_per_frame = (p.units_per_frame + 31) / 32;
     p.total_steps = (uint64_t)cnt * p.steps_per_frame;
-    p.xt = reinterpret_cast<const Tap*>(plan_taps);
-    p.dw = dw;
-    p.dh = dh;
-    p.area2x = area2x;
     uint64_t ctas = (p.total_steps + kWarps * 8 - 1) / (kWarps * 8);
     if (ctas > (uint64_t)sm_count()) ctas = sm_count();
     if (ctas < 1) ctas = 1;
     {
       LaunchScope ls("nv12_stream_kernel", st);
-      if (dst) nv12_stream_kernel<true><<<(unsigned)ctas, kThreads, kSmemBytes, st>>>(p, out + (size_t)i0 * 48);
-      else nv12_stream_kernel<false><<<(unsigned)ctas, kThreads, kSmemBytes, st>>>(p, out + (size_t)i0 * 48);
+      nv12_stream_kernel<<<(unsigned)ctas, kThreads, kSmemBytes, st>>>(p, out + (size_t)i0 * 48);
     }
     int rc = launch_status();
     if (rc) return rc;

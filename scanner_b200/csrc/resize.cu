@@ -9,20 +9,13 @@
 #include <math.h>
 #include <string.h>
 
+#include "resize_plan.cuh"
 #include "scn_common.cuh"
 
 namespace scn {
 namespace {
 
 constexpr int32_t kPlanMagic = 0x5243504c;  // "LPCR"
-
-struct PlanHeader {
-  int32_t magic, src_w, src_h, dst_w, dst_h, area2x, pad0, pad1;
-};
-// One tap entry per destination column / row: {src index 0, src index 1, weight 0, weight 1}
-struct Tap {
-  int32_t i0, i1, w0, w1;
-};
 
 void fill_taps(int ssz, int dsz, bool zero_weight_clamp, Tap* t) {
   const double inv_scale = (double)dsz / (double)ssz;

@@ -11,10 +11,6 @@ at the streaming kernel's edge geometries, and batches that the launchers split 
 Every comparison is exact: histograms against torch.bincount of v >> 4 (of kernels.nv12_to_rgb for NV12 surfaces,
 pinned to the reference's own kernel by test_ref_pin_gpu.py) or the closed form of a constant frame, Resize against
 kernels.resize of that RGB (pinned to the cv2 goldens) and the oracle on a sample."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
@@ -24,8 +20,6 @@ from oracle import synth
 from scanner_b200 import cabi, kernels
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 MAX_PTRS = 64                          # SCN_MAX_PTRS: frames per launch
 CSA_BLOCK, CSA_WARPS, CSA_MAX_BLOCKS = 6144, 8, 63   # hist_csa.cuh: kWarpBlock, kWarps, kMaxBlocks
@@ -73,7 +67,7 @@ def _csa_premise(n, nbytes):
 
 
 def _nvs_premise(n, h, w, pitch):
-    # nvs::eligible (nv12_stream.cuh:526-532); nvs::launch (nv12_stream.cuh:555-566): steps_per_frame =
+    # nvs::eligible (nv12_stream.cuh:382-388); nvs::launch (nv12_stream.cuh:409-416): steps_per_frame =
     # ceil(width / 16 * height / 2 / 32), ctas = ceil(total / (kWarps * 8)) capped at sm_count()
     assert w % 16 == 0 and pitch % 16 == 0 and h % 2 == 0 and w * h >= 64 * 1024
     spf = -(-(w // 16 * (h // 2)) // 32)
@@ -281,17 +275,13 @@ RESIZE_CASES = dict(LIMIT_CASES, **{
 })
 
 
-def _run_case(name):
+@pytest.mark.parametrize("name", list(RESIZE_CASES))
+def test_nv12_stream_saturating_surfaces(name):
     n, h, w, pitch, dw, dh = RESIZE_CASES[name]
     if name in LIMIT_CASES:
         _nvs_premise(n, h, w, pitch)
     surf, triples = _batch(n, h, w, pitch, seed=sum(map(ord, name)))
     _check_nv12(surf, w, h, dw, dh, triples, oracle_frames=(1, n - 1))
-
-
-@pytest.mark.parametrize("name", list(RESIZE_CASES))
-def test_nv12_stream_saturating_surfaces(name):
-    _run_case(name)
 
 
 @pytest.mark.parametrize("h,w,pitch,n,kernel", [(4096, 16, 16, 64, "nv12_stream_kernel"),
@@ -374,20 +364,3 @@ def test_small_frame_ops_over_64_frames():
     for i in range(n):
         assert (rgb[i] == oracle.nv12_to_rgb(host[i, :h], host[i, h:], w)).all(), i
 
-
-# ------------------------------------------------------------------- E. the other two Resize placements
-def _resize_mode_cases():
-    for name in RESIZE_CASES:
-        _run_case(name)
-        torch.cuda.empty_cache()
-
-
-@pytest.mark.parametrize("mode", ["fused", "split"])
-def test_resize_modes_at_the_limits(mode):
-    """SCN_NV12_RESIZE=fused produces the Resize rows inside the streaming pass (resize_units, tap_rgb), =split runs
-    nv12_resize_kernel behind it; both must equal the default.  The variable is read once per process."""
-    code = ("import sys; sys.path[:0] = ['.', 'tests']; import test_kernel_limits_gpu as T; T._resize_mode_cases(); "
-            "print('MODE_OK')")
-    out = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, SCN_NV12_RESIZE=mode), cwd=ROOT,
-                         capture_output=True, text=True)
-    assert "MODE_OK" in out.stdout, out.stdout[-2000:] + out.stderr[-3000:]

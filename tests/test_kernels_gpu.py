@@ -124,6 +124,28 @@ def test_blur_vs_oracle(h, w, k, n):
         assert (got[i] == oracle.blur(frames[i], k)).all()
 
 
+@pytest.mark.parametrize("h,w,k,kernel", [(64, 64, 3, "box_packed_kernel"), (64, 64, 5, "box_packed_kernel"),
+                                          (70, 1028, 3, "box3_kernel"), (70, 1028, 5, "box_generic_kernel"),
+                                          (33, 50, 3, "box_generic_kernel")])
+def test_blur_kernel_selection(h, w, k, kernel):
+    """16-byte aligned rows at least k tall take box_packed_kernel<K>, k = 3 included; otherwise k = 3 on 4-byte
+    aligned rows takes box3_kernel; everything else takes box_generic_kernel."""
+    frames = np.stack([synth.rand_frame(50 + i, h, w) for i in range(2)])
+    src = dev(frames)
+    L = cabi.lib()
+    L.scn_prof_enable(1)
+    try:
+        got = kernels.blur(src, k)
+        torch.cuda.synchronize()
+        ran = {name: v["launches"] for name, v in cabi.prof_report().items()}
+    finally:
+        L.scn_prof_enable(0)
+    assert ran == {kernel: 1}
+    got = got.cpu().numpy()
+    for i in range(2):
+        assert (got[i] == oracle.blur(frames[i], k)).all()
+
+
 def test_div9_multiply_shift_is_exact():
     """box3_kernel divides by 9 with (v * 7282) >> 16: exact for every reachable sum (<= 9*255)."""
     v = np.arange(0, 9 * 255 + 1, dtype=np.uint64)
@@ -285,10 +307,11 @@ def test_sharded_job_windows_on_one_gpu_equal_the_whole_clip():
 
 
 @pytest.mark.parametrize("h,w,k,n", [(480, 640, 5, 2), (2160, 3840, 5, 1), (1080, 1920, 9, 2), (70, 3088, 7, 2), (40, 1040, 31, 1),
-                                     (129, 1024, 4, 1), (257, 2064, 6, 2), (131, 48, 2, 3), (31, 16, 31, 1), (200, 1920, 16, 1)])
-def test_blur_streaming_kernel_vs_oracle(h, w, k, n):
-    """box_stream_kernel (bulk-async row ring, sliding sums): 16-byte aligned rows, several strips / row ranges,
-    even and odd kernel sizes (fl != fr), windows as tall as the frame."""
+                                     (129, 1024, 4, 1), (257, 2064, 6, 2), (131, 48, 2, 3), (31, 16, 31, 1), (200, 1920, 16, 1),
+                                     (90, 1040, 5, 2)])
+def test_blur_aligned_rows_vs_oracle(h, w, k, n):
+    """box_packed_kernel<K> on 16-byte aligned rows: several warps / strips / row ranges, even and odd kernel sizes
+    (fl != fr), windows as tall as the frame."""
     assert w % 16 == 0
     frames = np.stack([synth.rand_frame(60 + i, h, w) for i in range(n)])
     l0 = cabi.lib().scn_launch_count()
@@ -318,8 +341,9 @@ def test_blur_packed_kernel_every_size_vs_oracle(k):
 
 
 @pytest.mark.parametrize("k", [17, 18, 21, 24, 27, 30, 31])
-def test_blur_stream_kernel_large_sizes_vs_oracle(k):
-    """Kernel sizes above 16 (lane sums no longer fit u16) stay on box_stream_kernel."""
+def test_blur_packed_kernel_large_sizes_vs_oracle(k):
+    """Kernel sizes above 16, where box_packed_kernel<K> sums the terms in groups of 8 (a u16 lane no longer holds K
+    terms), on frames several warps wide with a saturated band."""
     frames = np.stack([synth.rand_frame(400 + k + i, 90, 1040) for i in range(2)])
     frames[1, 20:70] = 255
     got = kernels.blur(dev(frames), k).cpu().numpy()
@@ -328,26 +352,8 @@ def test_blur_stream_kernel_large_sizes_vs_oracle(k):
         assert (got[i] == want).all(), (k, i, np.argwhere(got[i] != want)[:4])
 
 
-def test_blur_stream_kernel_still_exact_when_selected():
-    """box_stream_kernel (bulk-async row ring) is no longer the default for any size; SCN_BLUR_PATH=stream selects it
-    (the variable is read once per process, hence the subprocess)."""
-    import subprocess
-    import sys
-    code = (
-        "import sys, numpy as np, torch; sys.path.insert(0, '.');"
-        "import oracle; from oracle import synth; from scanner_b200 import kernels, cabi;"
-        "\nfor (h, w, k) in [(90, 1040, 5), (70, 3088, 7), (40, 1040, 31), (129, 1024, 4), (131, 48, 2), (200, 1920, 16)]:"
-        "\n    f = np.stack([synth.rand_frame(7 * k + i, h, w) for i in range(2)])"
-        "\n    got = kernels.blur(torch.from_numpy(f).cuda(), k).cpu().numpy()"
-        "\n    assert all((got[i] == oracle.blur(f[i], k)).all() for i in range(2)), (h, w, k)"
-        "\nprint('STREAM_OK')")
-    out = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, SCN_BLUR_PATH="stream"),
-                         cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))), capture_output=True, text=True)
-    assert "STREAM_OK" in out.stdout, out.stdout[-2000:] + out.stderr[-2000:]
-
-
 def test_blur_division_by_multiply_shift_is_exact():
-    """box_stream_kernel divides a window sum by k*k with umulhi(v, floor(2^32 / k^2) + 1)."""
+    """box_packed_kernel<K> divides a window sum by k*k with umulhi(v, floor(2^32 / k^2) + 1)."""
     for k in range(2, 32):
         d = k * k
         v = np.arange(0, 255 * d + 1, dtype=np.uint64)

@@ -1,8 +1,7 @@
 #!/usr/bin/env python
 """CUDA-event timing of the box filter at BASELINE configs[2] size (16 x 4K frames) for several kernel sizes.
-SCN_BLUR3=stream routes kernel_size 3 through box_stream_kernel (default: box3_kernel).  One JSON line."""
+One JSON line."""
 import json
-import os
 import sys
 
 import torch
@@ -14,7 +13,7 @@ g = torch.Generator(device="cuda").manual_seed(3)
 n, h, w = 16, 2160, 3840
 frames = torch.randint(0, 256, (n, h, w, 3), dtype=torch.uint8, device="cuda", generator=g)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
-out = {"blur3_path": os.environ.get("SCN_BLUR3", "box3"), "path": os.environ.get("SCN_BLUR_PATH", "default")}
+out = {}
 for k in (3, 5, 7, 9, 15, 16, 17, 23, 31):
     kernels.blur(frames, k)
     ts = []
