@@ -160,12 +160,14 @@ __device__ __forceinline__ void ripple(Acc8<HI>& a, uint32_t c) {
   }
 }
 
-template <int HI>
-__device__ __forceinline__ void fold_step(Acc8<HI>& a, uint32_t c8, int step) {
-  if (step & 1) {
+// S = the step's index mod 4, known at compile time: a loop that runs steps in blocks of 4 folds without branches,
+// and pend3 / pend4 stay in fixed registers
+template <int S, int HI>
+__device__ __forceinline__ void fold_step(Acc8<HI>& a, uint32_t c8) {
+  if constexpr ((S & 1) != 0) {
     uint32_t c16;
     csa3(c16, a.hi[0], a.hi[0], a.pend3, c8);
-    if (step & 2) {
+    if constexpr ((S & 2) != 0) {
       uint32_t c32;
       csa3(c32, a.hi[1], a.hi[1], a.pend4, c16);
       ripple<2>(a, c32);
@@ -174,6 +176,18 @@ __device__ __forceinline__ void fold_step(Acc8<HI>& a, uint32_t c8, int step) {
     }
   } else {
     a.pend3 = c8;
+  }
+}
+
+template <int HI>
+__device__ __forceinline__ void fold_step(Acc8<HI>& a, uint32_t c8, int step) {
+  if (step & 1) {
+    if (step & 2)
+      fold_step<3>(a, c8);
+    else
+      fold_step<1>(a, c8);
+  } else {
+    fold_step<0>(a, c8);
   }
 }
 

@@ -8,6 +8,8 @@
 //   * surfaces are streamed with cp.async into a per-warp shared-memory ring (no load registers, the
 //     prefetch runs kStages-1 steps ahead across span and frame boundaries); a lane owns a "unit" of
 //     16 pixels x 2 rows per step (two luma rows, the chroma row and the next chroma row);
+//   * steps run in blocks of 4, so the fold of the carry-save carries has no run-time branches; the last steps
+//     of a frame and of a span run one at a time (see the span loop);
 //   * byte -> float on the XU pipe: `(float)((w >> 8k) & 0xff)` is I2F.U8 Rd, Rs.Bk -- no ALU work;
 //   * colour math on the FMA pipe.  Only the 4-bit bin reaches the histogram, so any arithmetic that
 //     yields the reference's bin for every input is exact by exhaustion (tests/test_ref_pin_gpu.py
@@ -193,7 +195,16 @@ struct Params {
   uint32_t units_per_frame;   // units_per_row * height / 2
   uint32_t steps_per_frame;   // ceil(units_per_frame / 32)
   uint64_t total_steps;
+  // a step moves a lane 32 units on: q = 32 / units_per_row row pairs and xs_step = 32 % units_per_row columns, plus
+  // one row pair more where the column wraps.  Its pointers move by 512 + (q + wrap) * (2 * pitch - width) bytes in
+  // the luma plane, 512 + (q + wrap) * (pitch - width) in the chroma plane (32 bits: see kMaxPitch)
+  uint32_t xs_step;
+  uint32_t inc_l, inc_l_wrap, inc_c, inc_c_wrap;
+  uint32_t fast_steps;        // leading steps of a frame whose 32 units all lie above the last chroma row
 };
+
+// bounds the per-step pointer increments above (< 512 + 33 * 2 * pitch) to 32 bits
+constexpr size_t kMaxPitch = (size_t)1 << 25;
 
 __device__ __forceinline__ uint32_t lane_count(const Acc& a, int lane) {
   uint32_t pl[kPlanes + 5];
@@ -209,6 +220,9 @@ __device__ __forceinline__ uint32_t lane_count(const Acc& a, int lane) {
 __device__ __forceinline__ void cp_async16(uint32_t smem_addr, const void* gptr, uint32_t src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_addr), "l"(gptr), "r"(src_bytes) : "memory");
 }
+__device__ __forceinline__ void cp_async16(uint32_t smem_addr, const void* gptr) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_addr), "l"(gptr) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() {
@@ -219,6 +233,11 @@ __device__ __forceinline__ uint4 lds128(uint32_t smem_addr) {
   asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(smem_addr));
   return r;
 }
+
+template <int J>
+struct Phase {
+  static constexpr int value = J;
+};
 
 static __global__ void __launch_bounds__(kThreads, 1)
 nv12_stream_kernel(const Params prm, int32_t* __restrict__ out) {
@@ -235,68 +254,60 @@ nv12_stream_kernel(const Params prm, int32_t* __restrict__ out) {
   // this lane's 16-byte slot in stage s, row k:  ring + ((s * 4 + k) * 32 + lane) * 16
   const uint32_t ring = (uint32_t)__cvta_generic_to_shared(smem_raw) + (uint32_t)warp * (kStages * 4 * 32 * 16) + lane * 16;
 
-  // ---- prefetch side: this lane's unit of the next step to fetch, tracked incrementally (pointers,
-  // not indices: the address arithmetic of a step is four 64-bit adds)
-  uint64_t pf_left = g_end - g_begin;                      // steps still to prefetch
+  // ring stage of global step g: g mod kStages, for the consumer and for the prefetch kStages - 1 steps ahead of it
+  auto slot_of = [&](uint32_t g) { return ring + (g & (kStages - 1)) * (4 * 32 * 16); };
+
+  // ---- prefetch side.  Two paths: fast_prefetch() serves the steps whose 32 lanes all read a unit of the frame
+  // above its last chroma row (all but the last few steps of a frame) with per-lane pointers it moves on by one
+  // select each; prefetch() serves any step (frame ends, padding lanes, the last chroma row, the range's end),
+  // locating the lane's unit from scratch.  The consumer picks the fast path a block of 4 steps at a time.
+  uint32_t pf_left = (uint32_t)(g_end - g_begin);         // steps still to prefetch
   uint32_t pf_frame = (uint32_t)(g_begin / prm.steps_per_frame);
   uint32_t pf_s = (uint32_t)(g_begin - (uint64_t)pf_frame * prm.steps_per_frame);
-  uint32_t pf_stage = (uint32_t)g_begin & (kStages - 1);
-  uint32_t pf_unit, pf_yp, pf_xs;                          // unit index in the frame, its row pair and column unit
+  uint32_t pf_fast = 0;                                    // steps from (pf_frame, pf_s) on that the fast path may take
+  uint32_t pf_xs;                                          // this lane's column unit in step (pf_frame, pf_s)
   const uint8_t *pf_l, *pf_c;                              // its luma / chroma 16-byte groups
-  auto locate = [&]() {
-    pf_unit = pf_s * 32u + (uint32_t)lane;
-    pf_yp = (uint32_t)(((uint64_t)pf_unit * prm.upr_recip) >> 32);   // == pf_unit / units_per_row
-    pf_xs = pf_unit - pf_yp * prm.units_per_row;
-    const bool active = pf_unit < prm.units_per_frame;     // lanes past the frame's last unit: any valid address
-    pf_l = prm.luma.p[pf_frame] + (active ? (size_t)(2 * pf_yp) * prm.pitch + (size_t)pf_xs * 16 : 0);
-    pf_c = prm.chroma.p[pf_frame] + (active ? (size_t)pf_yp * prm.pitch + (size_t)pf_xs * 16 : 0);
+  auto locate = [&](uint32_t& yp) {                        // returns whether the lane's unit lies in the frame
+    const uint32_t unit = pf_s * 32u + (uint32_t)lane;
+    yp = (uint32_t)(((uint64_t)unit * prm.upr_recip) >> 32);   // == unit / units_per_row
+    pf_xs = unit - yp * prm.units_per_row;
+    const bool active = unit < prm.units_per_frame;        // lanes past the frame's last unit: any valid address
+    pf_l = prm.luma.p[pf_frame] + (active ? (size_t)(2 * yp) * prm.pitch + (size_t)pf_xs * 16 : 0);
+    pf_c = prm.chroma.p[pf_frame] + (active ? (size_t)yp * prm.pitch + (size_t)pf_xs * 16 : 0);
+    return active;
   };
-  locate();
-  const size_t wrap_l = 2 * prm.pitch - (size_t)prm.units_per_row * 16, wrap_c = prm.pitch - (size_t)prm.units_per_row * 16;
-  auto prefetch = [&]() {
+  auto prefetch = [&](uint32_t slot) {
     if (pf_left) {
-      --pf_left;
-      const uint32_t nbytes = pf_unit < prm.units_per_frame ? 16u : 0u;  // 0: the slot is zero-filled, nothing is read
-      const size_t cnext = ((int)pf_yp < last_crow) ? prm.pitch : 0;
-      const uint32_t slot = ring + pf_stage * (4 * 32 * 16);
+      uint32_t yp;
+      const uint32_t nbytes = locate(yp) ? 16u : 0u;     // 0: the slot is zero-filled, nothing is read
+      const size_t cnext = ((int)yp < last_crow) ? prm.pitch : 0;
       cp_async16(slot, pf_l, nbytes);
       cp_async16(slot + 512, pf_l + prm.pitch, nbytes);
       cp_async16(slot + 1024, pf_c, nbytes);
       cp_async16(slot + 1536, pf_c + cnext, nbytes);
-      pf_stage = (pf_stage + 1) & (kStages - 1);
+      --pf_left;
       if (++pf_s == prm.steps_per_frame) {                 // next frame (warp-uniform, once per frame)
         pf_s = 0;
         ++pf_frame;
-        if (pf_left) locate();
-      } else {
-        pf_unit += 32;
-        pf_xs += 32;
-        pf_l += 512;
-        pf_c += 512;
-        if (prm.units_per_row >= 32) {                     // widths >= 512: at most one row-pair wrap per step
-          const bool wrap = pf_xs >= prm.units_per_row;
-          pf_xs -= wrap ? prm.units_per_row : 0u;
-          pf_yp += wrap ? 1u : 0u;
-          pf_l += wrap ? wrap_l : (size_t)0;
-          pf_c += wrap ? wrap_c : (size_t)0;
-        } else {
-          while (pf_xs >= prm.units_per_row) {
-            pf_xs -= prm.units_per_row;
-            ++pf_yp;
-            pf_l += wrap_l;
-            pf_c += wrap_c;
-          }
-        }
-        if (pf_unit >= prm.units_per_frame) {              // only in a frame's last step: any valid address
-          pf_l = prm.luma.p[pf_frame];
-          pf_c = prm.chroma.p[pf_frame];
-        }
       }
+      pf_fast = pf_s < prm.fast_steps ? min(prm.fast_steps - pf_s, pf_left) : 0u;
     }
     cp_async_commit();
   };
+  auto fast_prefetch = [&](uint32_t slot) {                // pointers valid (locate() at the start of a fast run)
+    cp_async16(slot, pf_l);
+    cp_async16(slot + 512, pf_l + prm.pitch);
+    cp_async16(slot + 1024, pf_c);
+    cp_async16(slot + 1536, pf_c + prm.pitch);
+    cp_async_commit();
+    pf_xs += prm.xs_step;                                  // < 2 * units_per_row: at most one wrap
+    const bool wrap = pf_xs >= prm.units_per_row;
+    pf_xs -= wrap ? prm.units_per_row : 0u;
+    pf_l += wrap ? prm.inc_l_wrap : prm.inc_l;
+    pf_c += wrap ? prm.inc_c_wrap : prm.inc_c;
+  };
 #pragma unroll
-  for (int i = 0; i < kStages - 1; ++i) prefetch();
+  for (int i = 0; i < kStages - 1; ++i) prefetch(slot_of((uint32_t)g_begin + i));
 
   uint64_t g0 = g_begin;
   while (g0 < g_end) {
@@ -314,15 +325,13 @@ nv12_stream_kernel(const Params prm, int32_t* __restrict__ out) {
       acc_clear(A[c]);
       acc_clear(B[c]);
     }
-    uint32_t padded_units = 0;
+    const uint32_t gs = (uint32_t)g0;   // step j of the span is global step gs + j
 
-    for (uint32_t step = 0; step < ns; ++step) {
-      prefetch();                    // step + kStages - 1
-      cp_async_wait<kStages - 1>();  // this step's group has landed (own bytes only: no barrier)
-      const uint32_t slot = ring + ((uint32_t)(g0 + step) & (kStages - 1)) * (4 * 32 * 16);
+    // one step's 32 pixels x 2 rows per lane (its group is the oldest in flight: wait for it, own bytes only, no
+    // barrier), counted into the accumulators; cA / cB get the weight-8 carries for the fold
+    auto count_step = [&](uint32_t slot, uint32_t (&cA)[3], uint32_t (&cB)[3]) {
+      cp_async_wait<kStages - 1>();
       const uint4 ya = lds128(slot), c0 = lds128(slot + 1024);
-      padded_units += ((s0 + step) * 32u + (uint32_t)lane < prm.units_per_frame) ? 0u : 1u;
-      uint32_t cA[3], cB[3];
       quad<0>(A, B, cA, cB, ya.x, c0.x, lut_lo);
       quad<1>(A, B, cA, cB, ya.y, c0.y, lut_lo);
       quad<2>(A, B, cA, cB, ya.z, c0.z, lut_lo);
@@ -333,10 +342,48 @@ nv12_stream_kernel(const Params prm, int32_t* __restrict__ out) {
       quad<5>(A, B, cA, cB, yb.y, avg4(c0.y, c1.y), lut_lo);
       quad<6>(A, B, cA, cB, yb.z, avg4(c0.z, c1.z), lut_lo);
       quad<7>(A, B, cA, cB, yb.w, avg4(c0.w, c1.w), lut_lo);
+    };
+    // step j of a block of 4.  Blocks start at span steps that are multiples of 4, so j is the fold's phase, and
+    // gs + j is the step's ring stage mod kStages
+    auto block_step = [&](auto phase) {
+      constexpr int j = decltype(phase)::value;
+      fast_prefetch(slot_of(gs + j + kStages - 1));
+      uint32_t cA[3], cB[3];
+      count_step(slot_of(gs + j), cA, cB);
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
-        fold_step(A[c], cA[c], (int)step);
-        fold_step(B[c], cB[c], (int)step);
+        fold_step<j>(A[c], cA[c]);
+        fold_step<j>(B[c], cB[c]);
+      }
+    };
+
+    uint32_t step = 0;
+    while (step < ns) {
+      if (ns - step >= 4 && pf_fast >= 4) {   // step is a multiple of 4 here
+        uint32_t yp;
+        locate(yp);
+        do {
+          block_step(Phase<0>{});
+          block_step(Phase<1>{});
+          block_step(Phase<2>{});
+          block_step(Phase<3>{});
+          step += 4;
+          pf_s += 4;
+          pf_left -= 4;
+          pf_fast -= 4;
+        } while (ns - step >= 4 && pf_fast >= 4);
+      } else {                                // single steps up to the next multiple of 4 or the span's end
+        do {
+          prefetch(slot_of(gs + step + kStages - 1));
+          uint32_t cA[3], cB[3];
+          count_step(slot_of(gs + step), cA, cB);
+#pragma unroll
+          for (int c = 0; c < 3; ++c) {
+            fold_step(A[c], cA[c], (int)step);
+            fold_step(B[c], cB[c], (int)step);
+          }
+          ++step;
+        } while (step < ns && (step & 3));
       }
     }
 
@@ -360,8 +407,9 @@ nv12_stream_kernel(const Params prm, int32_t* __restrict__ out) {
         if (cb) atomicAdd(&h[c * 16 + 8 + lane], (int)cb);
       }
     }
-    // padding units were fed as all-zero bytes: remove what 32 such pixels each contributed
-    const uint32_t pad_total = __reduce_add_sync(0xffffffffu, padded_units);
+    // padding units (the lanes past the frame's last unit in its last step) were fed as all-zero bytes: remove
+    // what 32 such pixels each contributed
+    const uint32_t pad_total = (s0 + ns == prm.steps_per_frame) ? prm.steps_per_frame * 32u - prm.units_per_frame : 0u;
     __syncwarp();
     if (pad_total && lane == 0) {
       const Rgb8 z = yuv_to_rgb(0, 0, 0);
@@ -381,7 +429,7 @@ nv12_stream_kernel(const Params prm, int32_t* __restrict__ out) {
 
 inline bool eligible(const uint8_t* const* lp, const uint8_t* const* cp, int n, size_t pitch, int width, int height) {
   if ((width & 15) || (pitch & 15) || (height & 1)) return false;
-  if ((size_t)width * height < 64 * 1024) return false;
+  if ((size_t)width * height < 64 * 1024 || pitch > kMaxPitch) return false;
   for (int i = 0; i < n; ++i)
     if ((reinterpret_cast<uintptr_t>(lp[i]) | reinterpret_cast<uintptr_t>(cp[i])) & 15) return false;
   return true;
@@ -411,6 +459,14 @@ inline int launch(const uint8_t* const* lp, const uint8_t* const* cp, int n, siz
     p.units_per_frame = p.units_per_row * (uint32_t)(height / 2);
     p.steps_per_frame = (p.units_per_frame + 31) / 32;
     p.total_steps = (uint64_t)cnt * p.steps_per_frame;
+    const uint32_t wrap_l = (uint32_t)(2 * pitch) - (uint32_t)width, wrap_c = (uint32_t)pitch - (uint32_t)width;
+    const uint32_t q = 32u / p.units_per_row;
+    p.xs_step = 32u % p.units_per_row;
+    p.inc_l = 512u + q * wrap_l;
+    p.inc_l_wrap = p.inc_l + wrap_l;
+    p.inc_c = 512u + q * wrap_c;
+    p.inc_c_wrap = p.inc_c + wrap_c;
+    p.fast_steps = (uint32_t)((uint64_t)(height / 2 - 1) * p.units_per_row / 32);
     uint64_t ctas = (p.total_steps + kWarps * 8 - 1) / (kWarps * 8);
     if (ctas > (uint64_t)sm_count()) ctas = sm_count();
     if (ctas < 1) ctas = 1;

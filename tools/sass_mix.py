@@ -1,7 +1,9 @@
 #!/usr/bin/env python3
 """Instruction mix of the loop that holds most of a kernel's conversions (I2F) / PRMTs, from `cuobjdump -sass`.
 
-    python tools/sass_mix.py scanner_b200/lib/libscn_kernels.so nv12_stream_kernelILb0 [anchor-mnemonic]
+    python tools/sass_mix.py scanner_b200/lib/libscn_kernels.so nv12_stream_kernel [anchor-mnemonic]
+
+nv12_stream_kernel's hot loop runs a block of 4 steps: divide its count by 4 for one 32-pixel step.
 """
 import collections
 import re
