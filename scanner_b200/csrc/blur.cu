@@ -330,28 +330,11 @@ int launch_blur(const uint8_t* const* sp, int n, int width, int height, int ksiz
   const int k = fl + fr + 1;
   const int in_w = TW + k - 1, in_h = TH + k - 1;
   const size_t smem = (((size_t)in_h * in_w * 3 + 15) & ~(size_t)15) + (size_t)in_h * TW * 3 * 2;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(box_generic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         100 * 1024);
-    if (e != cudaSuccess) return (int)e;
-    attr_set = true;
-  }
   if (((height + TH - 1) / TH) > 65535) return SCN_E_UNSUPPORTED;
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    PtrBatch s;
-    MutPtrBatch d;
-    bool aligned = (width % 4) == 0 && width >= 4 && height >= 3;
-    for (int i = 0; i < cnt; ++i) {
-      s.p[i] = sp[i0 + i];
-      d.p[i] = dp[i0 + i];
-      if (((uintptr_t)s.p[i] | (uintptr_t)d.p[i]) & 3) aligned = false;
-    }
-    bool aligned16 = (width % 16) == 0 && height >= k;
-    for (int i = 0; i < cnt; ++i)
-      if (((uintptr_t)s.p[i] | (uintptr_t)d.p[i]) & 15) aligned16 = false;
-    if (aligned16 && k >= 2) {
+  return for_each_chunk(n, [&](int i0, int cnt) {
+    const PtrBatch s = gather<PtrBatch>(sp, i0, cnt);
+    const MutPtrBatch d = gather<MutPtrBatch>(dp, i0, cnt);
+    if ((width % 16) == 0 && height >= k && k >= 2 && aligned(16, i0, cnt, sp, dp)) {
       const unsigned d2 = (unsigned)(k * k);
       const uint32_t magic = (uint32_t)((1ull << 32) / d2) + 1u;  // floor(v * magic / 2^32) == v / d2 for v <= 255 * d2
       const int quads = width * 3 / 16;
@@ -361,32 +344,30 @@ int launch_blur(const uint8_t* const* sp, int n, int width, int height, int ksiz
       int rows = 128;
       while (rows > 32 && (size_t)gx * ((height + rows - 1) / rows) * cnt < 2 * (size_t)sm_count()) rows >>= 1;
       dim3 grid(gx, (unsigned)((height + rows - 1) / rows), (unsigned)cnt);
-      LaunchScope ls("box_packed_kernel", st);
-      switch (k) {
+      return launch_kernel("box_packed_kernel", st, [&] {
+        switch (k) {
 #define SCN_BP_CASE(KK) \
   case KK: box_packed_kernel<KK><<<grid, BP_WARPS * 32, 0, st>>>(s, d, width, height, rows, magic); break;
-        SCN_BP_CASE(2) SCN_BP_CASE(3) SCN_BP_CASE(4) SCN_BP_CASE(5) SCN_BP_CASE(6) SCN_BP_CASE(7) SCN_BP_CASE(8)
-        SCN_BP_CASE(9) SCN_BP_CASE(10) SCN_BP_CASE(11) SCN_BP_CASE(12) SCN_BP_CASE(13) SCN_BP_CASE(14)
-        SCN_BP_CASE(15) SCN_BP_CASE(16) SCN_BP_CASE(17) SCN_BP_CASE(18) SCN_BP_CASE(19) SCN_BP_CASE(20) SCN_BP_CASE(21)
-        SCN_BP_CASE(22) SCN_BP_CASE(23) SCN_BP_CASE(24) SCN_BP_CASE(25) SCN_BP_CASE(26) SCN_BP_CASE(27) SCN_BP_CASE(28)
-        SCN_BP_CASE(29) SCN_BP_CASE(30) SCN_BP_CASE(31)
+          SCN_BP_CASE(2) SCN_BP_CASE(3) SCN_BP_CASE(4) SCN_BP_CASE(5) SCN_BP_CASE(6) SCN_BP_CASE(7) SCN_BP_CASE(8)
+          SCN_BP_CASE(9) SCN_BP_CASE(10) SCN_BP_CASE(11) SCN_BP_CASE(12) SCN_BP_CASE(13) SCN_BP_CASE(14)
+          SCN_BP_CASE(15) SCN_BP_CASE(16) SCN_BP_CASE(17) SCN_BP_CASE(18) SCN_BP_CASE(19) SCN_BP_CASE(20) SCN_BP_CASE(21)
+          SCN_BP_CASE(22) SCN_BP_CASE(23) SCN_BP_CASE(24) SCN_BP_CASE(25) SCN_BP_CASE(26) SCN_BP_CASE(27) SCN_BP_CASE(28)
+          SCN_BP_CASE(29) SCN_BP_CASE(30) SCN_BP_CASE(31)
 #undef SCN_BP_CASE
-      }
-    } else if (ksize == 3 && aligned) {
+        }
+      });
+    }
+    if (ksize == 3 && (width % 4) == 0 && width >= 4 && height >= 3 && aligned(4, i0, cnt, sp, dp)) {
       const int wpr = width * 3 / 4;
       dim3 grid((unsigned)((wpr + B3_THREADS - 1) / B3_THREADS), (unsigned)((height + B3_ROWS - 1) / B3_ROWS),
                 (unsigned)cnt);
-      LaunchScope ls("box3_kernel", st);
-      box3_kernel<<<grid, B3_THREADS, 0, st>>>(s, d, width, height, wpr);
-    } else {
-      dim3 grid((unsigned)((width + TW - 1) / TW), (unsigned)((height + TH - 1) / TH), (unsigned)cnt);
-      LaunchScope ls("box_generic_kernel", st);
-      box_generic_kernel<<<grid, BT, smem, st>>>(s, d, width, height, fl, fr);
+      return launch_kernel("box3_kernel", st, [&] { box3_kernel<<<grid, B3_THREADS, 0, st>>>(s, d, width, height, wpr); });
     }
-    int rc = launch_status();
-    if (rc) return rc;
-  }
-  return 0;
+    // at most 41,296 bytes of dynamic shared memory (k = 31): under the default limit
+    dim3 grid((unsigned)((width + TW - 1) / TW), (unsigned)((height + TH - 1) / TH), (unsigned)cnt);
+    return launch_kernel("box_generic_kernel", st,
+                         [&] { box_generic_kernel<<<grid, BT, smem, st>>>(s, d, width, height, fl, fr); });
+  });
 }
 
 }  // namespace
@@ -405,16 +386,6 @@ extern "C" int scn_box_blur_u8c3_strided(const uint8_t* src, size_t stride_bytes
   if (n < 0) return SCN_E_BADARG;
   if (n == 0) return 0;
   if (!src || !dst) return SCN_E_BADARG;
-  const uint8_t* sp[SCN_MAX_PTRS];
-  uint8_t* dp[SCN_MAX_PTRS];
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    for (int i = 0; i < cnt; ++i) {
-      sp[i] = src + (size_t)(i0 + i) * stride_bytes;
-      dp[i] = dst + (size_t)(i0 + i) * stride_bytes;
-    }
-    int rc = scn::launch_blur(sp, cnt, width, height, kernel_size, dp, (cudaStream_t)stream);
-    if (rc) return rc;
-  }
-  return 0;
+  return scn::launch_blur(scn::strided(src, stride_bytes, n).data(), n, width, height, kernel_size,
+                          scn::strided(dst, stride_bytes, n).data(), (cudaStream_t)stream);
 }

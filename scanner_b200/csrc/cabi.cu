@@ -5,6 +5,7 @@
 
 #include <map>
 #include <mutex>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -38,6 +39,24 @@ void prof_end(void* token, cudaStream_t st) {
   cudaEventRecord(r->b, st);
   std::lock_guard<std::mutex> g(g_prof_mu);
   g_recs.push_back(r);
+}
+
+int raise_smem_limit(const void* kernel, size_t bytes) {
+  static std::mutex mu;
+  static std::set<std::pair<const void*, int>> done;  // (kernel, device) pairs already raised
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) {
+    std::lock_guard<std::mutex> g(mu);
+    if (done.count({kernel, dev})) return 0;
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) {
+      done.insert({kernel, dev});
+      return 0;
+    }
+  }
+  cudaGetLastError();  // reported here, so that later calls report their own errors
+  return (int)e;
 }
 
 }  // namespace scn

@@ -259,23 +259,14 @@ int launch_u8(const uint8_t* const* src, uint8_t* const* dst, int n, uint32_t np
   const HsvTables tables = A == kHsv ? hsv_tables(code.hrange) : HsvTables{};
   // about two 16-pixel groups per thread
   const uint32_t want = (npix + 32u * kThreads - 1) / (32u * kThreads);
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    PtrBatch s;
-    MutPtrBatch d;
-    for (int i = 0; i < cnt; ++i) {
-      s.p[i] = src[i0 + i];
-      d.p[i] = dst[i0 + i];
-    }
+  return for_each_chunk(n, [&](int i0, int cnt) {
+    const PtrBatch s = gather<PtrBatch>(src, i0, cnt);
+    const MutPtrBatch d = gather<MutPtrBatch>(dst, i0, cnt);
     dim3 grid(want < 1 ? 1 : want, (unsigned)cnt);
-    {
-      LaunchScope ls("convert_color_kernel", st);
+    return launch_kernel("convert_color_kernel", st, [&] {
       convert_color_kernel<A, BGR><<<grid, kThreads, 0, st>>>(s, d, npix, code.hrange, tables);
-    }
-    const int rc = launch_status();
-    if (rc) return rc;
-  }
-  return 0;
+    });
+  });
 }
 
 template <Algo A, bool BGR>
@@ -283,27 +274,16 @@ int launch_nv12(const uint8_t* const* luma, const uint8_t* const* chroma, size_t
                 uint8_t* const* dst, const Code& code, cudaStream_t st) {
   const HsvTables tables = A == kHsv ? hsv_tables(code.hrange) : HsvTables{};
   const int units = (width + 15) / 16;
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    PtrBatch l, c;
-    MutPtrBatch d;
-    int vec = (width & 15) == 0 && (pitch & 15) == 0;
-    for (int i = 0; i < cnt; ++i) {
-      l.p[i] = luma[i0 + i];
-      c.p[i] = chroma[i0 + i];
-      d.p[i] = dst[i0 + i];
-      if (((uintptr_t)l.p[i] | (uintptr_t)c.p[i] | (uintptr_t)d.p[i]) & 15) vec = 0;
-    }
+  return for_each_chunk(n, [&](int i0, int cnt) {
+    const PtrBatch l = gather<PtrBatch>(luma, i0, cnt), c = gather<PtrBatch>(chroma, i0, cnt);
+    const MutPtrBatch d = gather<MutPtrBatch>(dst, i0, cnt);
+    const int vec = (width & 15) == 0 && (pitch & 15) == 0 && aligned(16, i0, cnt, luma, chroma, dst);
     dim3 grid((unsigned)((units + 127) / 128), (unsigned)height, (unsigned)cnt);
-    {
-      LaunchScope ls("convert_color_nv12_kernel", st);
+    return launch_kernel("convert_color_nv12_kernel", st, [&] {
       convert_color_nv12_kernel<A, BGR>
           <<<grid, 128, 0, st>>>(l, c, d, pitch, width, height, units, vec, code.hrange, tables);
-    }
-    const int rc = launch_status();
-    if (rc) return rc;
-  }
-  return 0;
+    });
+  });
 }
 
 }  // namespace

@@ -51,23 +51,15 @@ extern "C" int scn_frame_digest(const uint8_t* const* host_ptrs, int n, size_t b
   using namespace scn;
   if (n < 0 || (bytes & 3) || (n > 0 && (!host_ptrs || !out))) return SCN_E_BADARG;
   if (n == 0) return 0;
+  if (!aligned(4, 0, n, host_ptrs)) return SCN_E_BADARG;
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaMemsetAsync(out, 0, (size_t)n * 16, st);
   if (e != cudaSuccess) return (int)e;
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    PtrBatch b;
-    for (int i = 0; i < cnt; ++i) {
-      b.p[i] = host_ptrs[i0 + i];
-      if (reinterpret_cast<uintptr_t>(b.p[i]) & 3) return SCN_E_BADARG;
-    }
+  return for_each_chunk(n, [&](int i0, int cnt) {
+    const PtrBatch b = gather<PtrBatch>(host_ptrs, i0, cnt);
     dim3 grid((unsigned)(sm_count() * 4 / (cnt < 4 ? cnt : 4) + 1), (unsigned)(cnt < 4 ? cnt : 4));
-    {
-      LaunchScope ls("frame_digest_kernel", st);
+    return launch_kernel("frame_digest_kernel", st, [&] {
       frame_digest_kernel<<<grid, 256, 0, st>>>(b, cnt, bytes / 4, reinterpret_cast<unsigned long long*>(out) + 2 * i0);
-    }
-    const int rc = launch_status();
-    if (rc) return rc;
-  }
-  return 0;
+    });
+  });
 }

@@ -560,23 +560,20 @@ inline size_t gauss_smem(int r) { return ((size_t)(GTH + 2 * r) * (GTW + 2 * r) 
 inline size_t poly_smem(int n) { return ((size_t)(PTH + 2 * n) * (PTW + 2 * n) + (size_t)PTH * (PTW + 2 * n) * 3) * 4; }
 constexpr int kBoxMW = 7;  // the fused box kernel is instantiated for winSize 15 (the reference's)
 inline size_t box_smem(int m) { return (size_t)BTH * (((BTW + 2 * m) * 5) | 1) * 8; }
-// SCN_FLOW_UNFUSED=1 selects the two-pass kernels (kept as the reference the fused ones are tested against)
+// SCN_FLOW_UNFUSED=1 selects the two-pass kernels (kept as the reference the fused ones are tested against); they
+// also run on a device that refuses the fused kernels' shared-memory limit
 inline bool use_fused() {
-  static const bool v = [] {
+  static const bool off = [] {
     const char* e = getenv("SCN_FLOW_UNFUSED");
-    if (e && e[0] == '1') return false;
-    auto big = [](const void* f) {
-      return cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFusedSmemCap) == cudaSuccess;
-    };
-    return big((const void*)gauss_fused_kernel<0>) && big((const void*)gauss_fused_kernel<1>) &&
-           big((const void*)gauss_fused_kernel<4>) && big((const void*)gauss_fused_kernel<9>) &&
-           big((const void*)poly_fused_kernel<0>) && big((const void*)poly_fused_kernel<5>) &&
-           cudaFuncSetAttribute(box_solve_fused_kernel<kBoxMW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)kFusedSmemCap) == cudaSuccess &&
-           cudaFuncSetAttribute(box_solve_f32_kernel<kBoxMW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)kFusedSmemCap) == cudaSuccess;
+    return e && e[0] == '1';
   }();
-  return v;
+  if (off) return false;
+  for (const void* f : {(const void*)gauss_fused_kernel<0>, (const void*)gauss_fused_kernel<1>,
+                        (const void*)gauss_fused_kernel<4>, (const void*)gauss_fused_kernel<9>,
+                        (const void*)poly_fused_kernel<0>, (const void*)poly_fused_kernel<5>,
+                        (const void*)box_solve_fused_kernel<kBoxMW>, (const void*)box_solve_f32_kernel<kBoxMW>})
+    if (raise_smem_limit(f, kFusedSmemCap)) return false;
+  return true;
 }
 
 // ---- host-side constants --------------------------------------------------------------------
@@ -744,6 +741,7 @@ extern "C" int scn_farneback_u8c3_chain(const uint8_t* const* host_prev_ptrs, co
   if (workspace_bytes < scn_farneback_workspace_bytes(width, height)) return SCN_E_BADARG;
   if (height > 65535) return SCN_E_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
+  const bool fused = use_fused();
   Workspace ws;
   carve(workspace, width, height, &ws);
   Level lv[16];
@@ -761,7 +759,7 @@ extern "C" int scn_farneback_u8c3_chain(const uint8_t* const* host_prev_ptrs, co
     const int w = lv[k].w, h = lv[k].h;
     GaussK gk;
     make_gauss(lv[k].smooth, lv[k].sigma, gk);
-    if (use_fused() && gauss_smem(gk.radius) <= kFusedSmemCap) {
+    if (fused && gauss_smem(gk.radius) <= kFusedSmemCap) {
       LaunchScope ls("flow_gauss_fused_kernel", st);
       const dim3 gg((unsigned)((width + GTW - 1) / GTW), (unsigned)((height + GTH - 1) / GTH));
       const size_t sm = gauss_smem(gk.radius);
@@ -790,7 +788,7 @@ extern "C" int scn_farneback_u8c3_chain(const uint8_t* const* host_prev_ptrs, co
                                                       (double)height / h, 1.f);
       I = ws.I;
     }
-    if (use_fused() && poly_smem(pk.n) <= kFusedSmemCap) {
+    if (fused && poly_smem(pk.n) <= kFusedSmemCap) {
       LaunchScope ls("flow_poly_fused_kernel", st);
       const dim3 pg((unsigned)((w + PTW - 1) / PTW), (unsigned)((h + PTH - 1) / PTH));
       if (pk.n == 5) poly_fused_kernel<5><<<pg, FT, poly_smem(pk.n), st>>>(I, w, h, pk, dstR);
@@ -875,11 +873,11 @@ extern "C" int scn_farneback_u8c3_chain(const uint8_t* const* host_prev_ptrs, co
       }
       const int m = win_size / 2;
       for (int it = 0; it < num_iters; ++it) {
-        if (use_fused() && !box_in_f64() && m == kBoxMW && (size_t)w * h * 5 < ((size_t)1 << 31)) {
+        if (fused && !box_in_f64() && m == kBoxMW && (size_t)w * h * 5 < ((size_t)1 << 31)) {
           LaunchScope ls("flow_box_solve_f32_kernel", st);
           box_solve_f32_kernel<kBoxMW><<<dim3((unsigned)((w + B32W - 1) / B32W), (unsigned)((h + B32H - 1) / B32H)), FT,
                                          box32_smem(m), st>>>(ws.M, w, h, 1.0 / ((double)win_size * win_size), flow);
-        } else if (use_fused() && m == kBoxMW && (size_t)w * h * 5 < ((size_t)1 << 31)) {
+        } else if (fused && m == kBoxMW && (size_t)w * h * 5 < ((size_t)1 << 31)) {
           LaunchScope ls("flow_box_solve_fused_kernel", st);
           box_solve_fused_kernel<kBoxMW><<<dim3((unsigned)((w + BTW - 1) / BTW), (unsigned)((h + BTH - 1) / BTH)), FT,
                                            box_smem(m), st>>>(ws.M, w, h, 1.0 / ((double)win_size * win_size), flow);

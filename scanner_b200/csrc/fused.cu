@@ -184,13 +184,6 @@ extern "C" int scn_nv12_hist_resize(const uint8_t* const* host_luma_ptrs,
     if (e != cudaSuccess) return (int)e;
   }
   const int quads = (width + 3) / 4;
-  // Large aligned surfaces take the streaming histogram kernel (nv12_stream.cuh); tiny, ragged or unaligned ones
-  // take nv12_hist_kernel.  Resize is nv12_resize_kernel either way.
-  bool stream_ok = do_hist;
-  for (int i0 = 0; i0 < n && stream_ok; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    stream_ok = nvs::eligible(host_luma_ptrs + i0, host_chroma_ptrs + i0, cnt, pitch, width, height);
-  }
   // Histogram and Resize together: the Resize kernels go to the side stream (see SideStream), forked before any
   // histogram kernel is enqueued so that both can be resident together
   SideStream* side = nullptr;
@@ -203,42 +196,35 @@ extern "C" int scn_nv12_hist_resize(const uint8_t* const* host_luma_ptrs,
       rst = side->stream;
     }
   }
-  int rc = stream_ok ? nvs::launch(host_luma_ptrs, host_chroma_ptrs, n, pitch, width, height, hist_out, st) : 0;
-  // the generic histogram and the Resize, per chunk of 64 surfaces
-  for (int i0 = 0; i0 < n && rc == 0 && (do_resize || !stream_ok); i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    PtrBatch l, c;
-    MutPtrBatch d;
-    int vec_ok = ((pitch & 3) == 0);
-    for (int i = 0; i < cnt; ++i) {
-      l.p[i] = host_luma_ptrs[i0 + i];
-      c.p[i] = host_chroma_ptrs[i0 + i];
-      d.p[i] = do_resize ? host_dst_ptrs[i0 + i] : nullptr;
-      if (((uintptr_t)l.p[i] | (uintptr_t)c.p[i]) & 3) vec_ok = 0;
-    }
-    if (do_hist && !stream_ok) {
-      const int gx = (quads + HT - 1) / HT;
-      int gy = (sm_count() * 8 + gx * cnt - 1) / (gx * cnt);
-      if (gy < 1) gy = 1;
-      if (gy > height) gy = height;
-      dim3 grid((unsigned)gx, (unsigned)gy, (unsigned)cnt);
-      {
-        LaunchScope ls("nv12_hist_kernel", st);
-        nv12_hist_kernel<<<grid, HT, 0, st>>>(l, c, pitch, width, height, quads, vec_ok, hist_out + (size_t)i0 * 48);
+  const int rc = for_each_chunk(n, [&](int i0, int cnt) {
+    const PtrBatch l = gather<PtrBatch>(host_luma_ptrs, i0, cnt), c = gather<PtrBatch>(host_chroma_ptrs, i0, cnt);
+    if (do_hist) {
+      // Large aligned surfaces take the streaming histogram kernel (nv12_stream.cuh); tiny, ragged or unaligned ones
+      // take nv12_hist_kernel.  Resize is nv12_resize_kernel either way.
+      int32_t* o = hist_out + (size_t)i0 * 48;
+      int hrc;
+      if (nvs::eligible(host_luma_ptrs, host_chroma_ptrs, i0, cnt, pitch, width, height)) {
+        hrc = nvs::launch(l, c, cnt, pitch, width, height, o, st);
+      } else {
+        const int vec_ok = (pitch & 3) == 0 && aligned(4, i0, cnt, host_luma_ptrs, host_chroma_ptrs);
+        const int gx = (quads + HT - 1) / HT;
+        int gy = (sm_count() * 8 + gx * cnt - 1) / (gx * cnt);
+        if (gy < 1) gy = 1;
+        if (gy > height) gy = height;
+        dim3 grid((unsigned)gx, (unsigned)gy, (unsigned)cnt);
+        hrc = launch_kernel("nv12_hist_kernel", st, [&] {
+          nv12_hist_kernel<<<grid, HT, 0, st>>>(l, c, pitch, width, height, quads, vec_ok, o);
+        });
       }
-      rc = launch_status();
-      if (rc) break;
+      if (hrc || !do_resize) return hrc;
     }
-    if (do_resize) {
-      dim3 g2((unsigned)((dst_w * dst_h + 255) / 256), (unsigned)cnt);
-      {
-        LaunchScope ls("nv12_resize_kernel", rst);
-        nv12_resize_kernel<<<g2, 256, 0, rst>>>(l, c, pitch, width, height, d, (const uint8_t*)plan, dst_w, dst_h,
-                                              area2x ? 1 : 0);
-      }
-      rc = launch_status();
-    }
-  }
+    const MutPtrBatch d = gather<MutPtrBatch>(host_dst_ptrs, i0, cnt);
+    dim3 g2((unsigned)((dst_w * dst_h + 255) / 256), (unsigned)cnt);
+    return launch_kernel("nv12_resize_kernel", rst, [&] {
+      nv12_resize_kernel<<<g2, 256, 0, rst>>>(l, c, pitch, width, height, d, (const uint8_t*)plan, dst_w, dst_h,
+                                            area2x ? 1 : 0);
+    });
+  });
   // join, also on the error path: the caller's stream must not run ahead of the side stream
   if (side) {
     if (cudaEventRecord(side->join, side->stream) != cudaSuccess || cudaStreamWaitEvent(st, side->join, 0) != cudaSuccess) {

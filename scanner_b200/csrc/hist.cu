@@ -83,27 +83,20 @@ int launch_hist(const uint8_t* const* ptrs, int n, int width, int height, int32_
   if (e != cudaSuccess) return (int)e;
   if (nbytes == 0) return 0;
 
-  if (csa::eligible(ptrs, n, nbytes)) return csa::launch(ptrs, n, nbytes, out, st);
-
-  // grid.x: enough 256-thread blocks to give every thread ~8 vectors, capped so the whole
-  // launch is a few waves of the SM array.
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    PtrBatch pb;
-    for (int i = 0; i < cnt; ++i) pb.p[i] = ptrs[i0 + i];
+  return for_each_chunk(n, [&](int i0, int cnt) {
+    const PtrBatch pb = gather<PtrBatch>(ptrs, i0, cnt);
+    int32_t* o = out + (size_t)i0 * 48;
+    if (csa::eligible(ptrs, i0, cnt, nbytes)) return csa::launch(pb, cnt, nbytes, o, st);
+    // grid.x: enough 256-thread blocks to give every thread ~8 vectors, capped so the whole
+    // launch is a few waves of the SM array.
     size_t want = (nbytes / 16 + (size_t)kGenThreads * 8 - 1) / ((size_t)kGenThreads * 8);
     if (want < 1) want = 1;
     size_t cap = (size_t)(sm_count() * 8 + cnt - 1) / cnt;
     if (cap < 1) cap = 1;
     dim3 grid((unsigned)(want < cap ? want : cap), (unsigned)cnt);
-    {
-      LaunchScope ls("hist16_generic_kernel", st);
-      hist16_generic_kernel<<<grid, kGenThreads, 0, st>>>(pb, nbytes, out + (size_t)i0 * 48);
-    }
-    int rc = launch_status();
-    if (rc) return rc;
-  }
-  return 0;
+    return launch_kernel("hist16_generic_kernel", st,
+                         [&] { hist16_generic_kernel<<<grid, kGenThreads, 0, st>>>(pb, nbytes, o); });
+  });
 }
 
 }  // namespace
@@ -119,13 +112,5 @@ extern "C" int scn_hist16_u8c3_strided(const uint8_t* base, size_t stride_bytes,
   if (n < 0) return SCN_E_BADARG;
   if (n == 0) return 0;
   if (!base) return SCN_E_BADARG;
-  const uint8_t* ptrs[SCN_MAX_PTRS];
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    for (int i = 0; i < cnt; ++i) ptrs[i] = base + (size_t)(i0 + i) * stride_bytes;
-    int rc = scn::launch_hist(ptrs, cnt, width, height, out + (size_t)i0 * 48,
-                              (cudaStream_t)stream);
-    if (rc) return rc;
-  }
-  return 0;
+  return scn::launch_hist(scn::strided(base, stride_bytes, n).data(), n, width, height, out, (cudaStream_t)stream);
 }

@@ -215,36 +215,26 @@ hist16_csa_kernel(const Params prm, int32_t* __restrict__ out) {
   }
 }
 
-inline bool eligible(const uint8_t* const* ptrs, int n, size_t nbytes) {
+// Whether frames [i0, i0 + cnt) of `ptrs` can take hist16_csa_kernel.
+inline bool eligible(const uint8_t* const* ptrs, int i0, int cnt, size_t nbytes) {
   if (nbytes < (size_t)kWarpBlock * 8) return false;
   if (nbytes / kWarpBlock > 0xFFFFFFFFull) return false;
-  for (int i = 0; i < n; ++i)
-    if (reinterpret_cast<uintptr_t>(ptrs[i]) & 15) return false;
-  return true;
+  return aligned(16, i0, cnt, ptrs);
 }
 
-// `out` must already be zeroed (launch_hist memsets it).
-inline int launch(const uint8_t* const* ptrs, int n, size_t nbytes, int32_t* out, cudaStream_t st) {
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    Params p;
-    for (int i = 0; i < cnt; ++i) p.frames.p[i] = ptrs[i0 + i];
-    p.n = cnt;
-    p.blocks_per_frame = (uint32_t)(nbytes / kWarpBlock);
-    p.tail_bytes = (uint32_t)(nbytes - (size_t)p.blocks_per_frame * kWarpBlock);
-    p.total_blocks = (uint64_t)cnt * p.blocks_per_frame;
-    // persistent: one CTA per SM; with little work use fewer CTAs so every warp gets >= 4 blocks
-    uint64_t ctas = (p.total_blocks + kWarps * 4 - 1) / (kWarps * 4);
-    if (ctas > (uint64_t)sm_count()) ctas = sm_count();
-    if (ctas < 1) ctas = 1;
-    {
-      LaunchScope ls("hist16_csa_kernel", st);
-      hist16_csa_kernel<<<(unsigned)ctas, kThreads, 0, st>>>(p, out + (size_t)i0 * 48);
-    }
-    int rc = launch_status();
-    if (rc) return rc;
-  }
-  return 0;
+// One launch over the `n` frames of `frames`.  `out` must already be zeroed (launch_hist memsets it).
+inline int launch(const PtrBatch& frames, int n, size_t nbytes, int32_t* out, cudaStream_t st) {
+  Params p;
+  p.frames = frames;
+  p.n = n;
+  p.blocks_per_frame = (uint32_t)(nbytes / kWarpBlock);
+  p.tail_bytes = (uint32_t)(nbytes - (size_t)p.blocks_per_frame * kWarpBlock);
+  p.total_blocks = (uint64_t)n * p.blocks_per_frame;
+  // persistent: one CTA per SM; with little work use fewer CTAs so every warp gets >= 4 blocks
+  uint64_t ctas = (p.total_blocks + kWarps * 4 - 1) / (kWarps * 4);
+  if (ctas > (uint64_t)sm_count()) ctas = sm_count();
+  if (ctas < 1) ctas = 1;
+  return launch_kernel("hist16_csa_kernel", st, [&] { hist16_csa_kernel<<<(unsigned)ctas, kThreads, 0, st>>>(p, out); });
 }
 
 }  // namespace csa

@@ -168,30 +168,19 @@ extern "C" int scn_nv12_pack(const uint8_t* const* host_luma_ptrs, const uint8_t
   if (n == 0) return 0;
   if (!host_luma_ptrs || !host_chroma_ptrs || !host_dst_ptrs) return SCN_E_BADARG;
   cudaStream_t st = (cudaStream_t)stream;
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    PtrBatch l, c;
-    MutPtrBatch d;
-    int vec16 = ((pitch & 15) == 0) && ((width & 15) == 0);
-    for (int i = 0; i < cnt; ++i) {
-      l.p[i] = host_luma_ptrs[i0 + i];
-      c.p[i] = host_chroma_ptrs[i0 + i];
-      d.p[i] = host_dst_ptrs[i0 + i];
-      if (((uintptr_t)l.p[i] | (uintptr_t)c.p[i] | (uintptr_t)d.p[i]) & 15) vec16 = 0;
-    }
+  return for_each_chunk(n, [&](int i0, int cnt) {
+    const PtrBatch l = gather<PtrBatch>(host_luma_ptrs, i0, cnt), c = gather<PtrBatch>(host_chroma_ptrs, i0, cnt);
+    const MutPtrBatch d = gather<MutPtrBatch>(host_dst_ptrs, i0, cnt);
+    const int vec16 = ((pitch & 15) == 0) && ((width & 15) == 0) &&
+                      aligned(16, i0, cnt, host_luma_ptrs, host_chroma_ptrs, host_dst_ptrs);
     const long work = vec16 ? (long)(width >> 4) * (height + height / 2) : (long)width * (height + height / 2);
     long gx = (work + 255) / 256;
     const long cap = (long)sm_count() * 8 / cnt + 1;
     if (gx > cap) gx = cap;
     dim3 grid((unsigned)gx, 1, (unsigned)cnt);
-    {
-      LaunchScope ls("nv12_pack_kernel", st);
-      nv12_pack_kernel<<<grid, 256, 0, st>>>(l, c, d, pitch, width, height, vec16);
-    }
-    int rc = launch_status();
-    if (rc) return rc;
-  }
-  return 0;
+    return launch_kernel("nv12_pack_kernel", st,
+                         [&] { nv12_pack_kernel<<<grid, 256, 0, st>>>(l, c, d, pitch, width, height, vec16); });
+  });
 }
 
 extern "C" int scn_nv12_to_rgb24(const uint8_t* const* host_luma_ptrs,
@@ -207,33 +196,22 @@ extern "C" int scn_nv12_to_rgb24(const uint8_t* const* host_luma_ptrs,
   if (height > 65535) return SCN_E_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
   const int quads = (width + 3) / 4;
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    PtrBatch l, c;
-    MutPtrBatch r;
-    int vec_ok = ((pitch & 3) == 0) && ((rgb_pitch & 3) == 0);
-    for (int i = 0; i < cnt; ++i) {
-      l.p[i] = host_luma_ptrs[i0 + i];
-      c.p[i] = host_chroma_ptrs[i0 + i];
-      r.p[i] = host_rgb_ptrs[i0 + i];
-      if (((uintptr_t)l.p[i] | (uintptr_t)c.p[i] | (uintptr_t)r.p[i]) & 3) vec_ok = 0;
-    }
-    int vec16 = ((width & 15) == 0) && ((pitch & 15) == 0) && ((rgb_pitch & 15) == 0);
-    for (int i = 0; i < cnt; ++i)
-      if (((uintptr_t)l.p[i] | (uintptr_t)c.p[i] | (uintptr_t)r.p[i]) & 15) vec16 = 0;
-    if (vec16) {
+  return for_each_chunk(n, [&](int i0, int cnt) {
+    const PtrBatch l = gather<PtrBatch>(host_luma_ptrs, i0, cnt), c = gather<PtrBatch>(host_chroma_ptrs, i0, cnt);
+    const MutPtrBatch r = gather<MutPtrBatch>(host_rgb_ptrs, i0, cnt);
+    if (((width & 15) == 0) && ((pitch & 15) == 0) && ((rgb_pitch & 15) == 0) &&
+        aligned(16, i0, cnt, host_luma_ptrs, host_chroma_ptrs, host_rgb_ptrs)) {
       const int units = width / 16;
       dim3 grid((unsigned)((units + 127) / 128), (unsigned)height, (unsigned)cnt);
-      LaunchScope ls("nv12_to_rgb_kernel", st);
-      nv12_to_rgb16_kernel<<<grid, 128, 0, st>>>(l, c, r, pitch, height, rgb_pitch, units);
-    } else {
-      dim3 grid((unsigned)((quads + 255) / 256), (unsigned)height, (unsigned)cnt);
-      LaunchScope ls("nv12_to_rgb_kernel", st);
-      nv12_to_rgb_kernel<<<grid, 256, 0, st>>>(l, c, r, pitch, width, height, rgb_pitch, quads,
-                                             vec_ok);
+      return launch_kernel("nv12_to_rgb16_kernel", st, [&] {
+        nv12_to_rgb16_kernel<<<grid, 128, 0, st>>>(l, c, r, pitch, height, rgb_pitch, units);
+      });
     }
-    int rc = launch_status();
-    if (rc) return rc;
-  }
-  return 0;
+    const int vec_ok = ((pitch & 3) == 0) && ((rgb_pitch & 3) == 0) &&
+                       aligned(4, i0, cnt, host_luma_ptrs, host_chroma_ptrs, host_rgb_ptrs);
+    dim3 grid((unsigned)((quads + 255) / 256), (unsigned)height, (unsigned)cnt);
+    return launch_kernel("nv12_to_rgb_kernel", st, [&] {
+      nv12_to_rgb_kernel<<<grid, 256, 0, st>>>(l, c, r, pitch, width, height, rgb_pitch, quads, vec_ok);
+    });
+  });
 }

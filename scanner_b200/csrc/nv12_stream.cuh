@@ -427,57 +427,43 @@ nv12_stream_kernel(const Params prm, int32_t* __restrict__ out) {
   cp_async_wait<0>();
 }
 
-inline bool eligible(const uint8_t* const* lp, const uint8_t* const* cp, int n, size_t pitch, int width, int height) {
+// Whether surfaces [i0, i0 + cnt) of `lp` / `cp` can take nv12_stream_kernel.
+inline bool eligible(const uint8_t* const* lp, const uint8_t* const* cp, int i0, int cnt, size_t pitch, int width,
+                     int height) {
   if ((width & 15) || (pitch & 15) || (height & 1)) return false;
   if ((size_t)width * height < 64 * 1024 || pitch > kMaxPitch) return false;
-  for (int i = 0; i < n; ++i)
-    if ((reinterpret_cast<uintptr_t>(lp[i]) | reinterpret_cast<uintptr_t>(cp[i])) & 15) return false;
-  return true;
+  return aligned(16, i0, cnt, lp, cp);
 }
 
-// `out` must already be zeroed.
-inline int launch(const uint8_t* const* lp, const uint8_t* const* cp, int n, size_t pitch, int width, int height,
+// One launch over the `n` surfaces of `luma` / `chroma`.  `out` must already be zeroed.
+inline int launch(const PtrBatch& luma, const PtrBatch& chroma, int n, size_t pitch, int width, int height,
                   int32_t* out, cudaStream_t st) {
-  static std::atomic<int> attr_done{0};
-  if (!attr_done.load(std::memory_order_acquire)) {
-    const cudaError_t e = cudaFuncSetAttribute(nv12_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e != cudaSuccess) return (int)e;
-    attr_done.store(1, std::memory_order_release);
-  }
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    Params p;
-    for (int i = 0; i < cnt; ++i) {
-      p.luma.p[i] = lp[i0 + i];
-      p.chroma.p[i] = cp[i0 + i];
-    }
-    p.pitch = pitch;
-    p.width = width;
-    p.height = height;
-    p.units_per_row = (uint32_t)(width / 16);
-    p.upr_recip = (1ull << 32) / p.units_per_row + 1u;
-    p.units_per_frame = p.units_per_row * (uint32_t)(height / 2);
-    p.steps_per_frame = (p.units_per_frame + 31) / 32;
-    p.total_steps = (uint64_t)cnt * p.steps_per_frame;
-    const uint32_t wrap_l = (uint32_t)(2 * pitch) - (uint32_t)width, wrap_c = (uint32_t)pitch - (uint32_t)width;
-    const uint32_t q = 32u / p.units_per_row;
-    p.xs_step = 32u % p.units_per_row;
-    p.inc_l = 512u + q * wrap_l;
-    p.inc_l_wrap = p.inc_l + wrap_l;
-    p.inc_c = 512u + q * wrap_c;
-    p.inc_c_wrap = p.inc_c + wrap_c;
-    p.fast_steps = (uint32_t)((uint64_t)(height / 2 - 1) * p.units_per_row / 32);
-    uint64_t ctas = (p.total_steps + kWarps * 8 - 1) / (kWarps * 8);
-    if (ctas > (uint64_t)sm_count()) ctas = sm_count();
-    if (ctas < 1) ctas = 1;
-    {
-      LaunchScope ls("nv12_stream_kernel", st);
-      nv12_stream_kernel<<<(unsigned)ctas, kThreads, kSmemBytes, st>>>(p, out + (size_t)i0 * 48);
-    }
-    int rc = launch_status();
-    if (rc) return rc;
-  }
-  return 0;
+  const int e = raise_smem_limit((const void*)nv12_stream_kernel, kSmemBytes);
+  if (e) return e;
+  Params p;
+  p.luma = luma;
+  p.chroma = chroma;
+  p.pitch = pitch;
+  p.width = width;
+  p.height = height;
+  p.units_per_row = (uint32_t)(width / 16);
+  p.upr_recip = (1ull << 32) / p.units_per_row + 1u;
+  p.units_per_frame = p.units_per_row * (uint32_t)(height / 2);
+  p.steps_per_frame = (p.units_per_frame + 31) / 32;
+  p.total_steps = (uint64_t)n * p.steps_per_frame;
+  const uint32_t wrap_l = (uint32_t)(2 * pitch) - (uint32_t)width, wrap_c = (uint32_t)pitch - (uint32_t)width;
+  const uint32_t q = 32u / p.units_per_row;
+  p.xs_step = 32u % p.units_per_row;
+  p.inc_l = 512u + q * wrap_l;
+  p.inc_l_wrap = p.inc_l + wrap_l;
+  p.inc_c = 512u + q * wrap_c;
+  p.inc_c_wrap = p.inc_c + wrap_c;
+  p.fast_steps = (uint32_t)((uint64_t)(height / 2 - 1) * p.units_per_row / 32);
+  uint64_t ctas = (p.total_steps + kWarps * 8 - 1) / (kWarps * 8);
+  if (ctas > (uint64_t)sm_count()) ctas = sm_count();
+  if (ctas < 1) ctas = 1;
+  return launch_kernel("nv12_stream_kernel", st,
+                       [&] { nv12_stream_kernel<<<(unsigned)ctas, kThreads, kSmemBytes, st>>>(p, out); });
 }
 
 }  // namespace nvs

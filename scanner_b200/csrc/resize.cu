@@ -92,26 +92,17 @@ int launch_resize(const uint8_t* const* sp, int n, int sw, int sh, uint8_t* cons
   if (!sp || !dp) return SCN_E_BADARG;
   const bool area2x = (sw == 2 * dw && sh == 2 * dh);
   if (!area2x && !plan) return SCN_E_PLAN;
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    PtrBatch s;
-    MutPtrBatch d;
-    for (int i = 0; i < cnt; ++i) {
-      s.p[i] = sp[i0 + i];
-      d.p[i] = dp[i0 + i];
-    }
+  return for_each_chunk(n, [&](int i0, int cnt) {
+    const PtrBatch s = gather<PtrBatch>(sp, i0, cnt);
+    const MutPtrBatch d = gather<MutPtrBatch>(dp, i0, cnt);
     dim3 grid((unsigned)((dw * dh + 255) / 256), (unsigned)cnt);
-    if (area2x) {
-      LaunchScope ls("resize_area2x_kernel", st);
-      resize_area2x_kernel<<<grid, 256, 0, st>>>(s, d, sw, dw, dh);
-    } else {
-      LaunchScope ls("resize_linear_kernel", st);
+    if (area2x)
+      return launch_kernel("resize_area2x_kernel", st,
+                           [&] { resize_area2x_kernel<<<grid, 256, 0, st>>>(s, d, sw, dw, dh); });
+    return launch_kernel("resize_linear_kernel", st, [&] {
       resize_linear_kernel<<<grid, 256, 0, st>>>(s, d, (const uint8_t*)plan, sw, dw, dh);
-    }
-    int rc = launch_status();
-    if (rc) return rc;
-  }
-  return 0;
+    });
+  });
 }
 
 }  // namespace scn
@@ -171,17 +162,6 @@ extern "C" int scn_resize_bilinear_u8c3_strided(const uint8_t* src, size_t src_s
   if (n < 0) return SCN_E_BADARG;
   if (n == 0) return 0;
   if (!src || !dst) return SCN_E_BADARG;
-  const uint8_t* sp[SCN_MAX_PTRS];
-  uint8_t* dp[SCN_MAX_PTRS];
-  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
-    const int cnt = (n - i0 < SCN_MAX_PTRS) ? (n - i0) : SCN_MAX_PTRS;
-    for (int i = 0; i < cnt; ++i) {
-      sp[i] = src + (size_t)(i0 + i) * src_stride;
-      dp[i] = dst + (size_t)(i0 + i) * dst_stride;
-    }
-    int rc = scn::launch_resize(sp, cnt, src_w, src_h, dp, dst_w, dst_h, plan,
-                                (cudaStream_t)stream);
-    if (rc) return rc;
-  }
-  return 0;
+  return scn::launch_resize(scn::strided(src, src_stride, n).data(), n, src_w, src_h,
+                            scn::strided(dst, dst_stride, n).data(), dst_w, dst_h, plan, (cudaStream_t)stream);
 }

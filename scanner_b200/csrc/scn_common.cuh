@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include <atomic>
+#include <vector>
 
 #include "scn_kernels.h"
 
@@ -59,6 +60,58 @@ inline int launch_status() {
   }
   return 0;
 }
+
+// ---- the host side every batched entry point shares ----
+
+// Calls launch(i0, cnt) for each run [i0, i0 + cnt) of at most SCN_MAX_PTRS frames of a batch of n, in order, and
+// returns the first nonzero status; the runs after it are not enqueued.
+template <class F>
+inline int for_each_chunk(int n, F&& launch) {
+  for (int i0 = 0; i0 < n; i0 += SCN_MAX_PTRS) {
+    const int rc = launch(i0, n - i0 < SCN_MAX_PTRS ? n - i0 : SCN_MAX_PTRS);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+// Pointers [i0, i0 + cnt) of a host array (cnt <= SCN_MAX_PTRS) as a PtrBatch or MutPtrBatch.
+template <class Batch, class P>
+inline Batch gather(const P* ptrs, int i0, int cnt) {
+  Batch b;
+  for (int i = 0; i < cnt; ++i) b.p[i] = ptrs[i0 + i];
+  return b;
+}
+
+// Whether pointers [i0, i0 + cnt) of every host array are multiples of `align` (a power of two) bytes.
+template <class... P>
+inline bool aligned(uintptr_t align, int i0, int cnt, const P*... arrays) {
+  uintptr_t bits = 0;
+  for (int i = i0; i < i0 + cnt; ++i) bits |= (reinterpret_cast<uintptr_t>(arrays[i]) | ...);
+  return (bits & (align - 1)) == 0;
+}
+
+// base, base + stride, ... : n frames of a dense batch as a host pointer array.
+template <class T>
+inline std::vector<T*> strided(T* base, size_t stride, int n) {
+  std::vector<T*> p((size_t)n);
+  for (int i = 0; i < n; ++i) p[i] = base + (size_t)i * stride;
+  return p;
+}
+
+// Enqueues one launch under `name` (the launch counter and scn_prof_* see it by that name) and returns its status.
+template <class F>
+inline int launch_kernel(const char* name, cudaStream_t st, F&& enqueue) {
+  {
+    LaunchScope ls(name, st);
+    enqueue();
+  }
+  return launch_status();
+}
+
+// Raises `kernel`'s dynamic shared-memory limit to `bytes` on the current device.  Function attributes belong to a
+// device's context, so this is done once per (kernel, device); safe to call from any thread.  Each kernel is given
+// one limit.
+int raise_smem_limit(const void* kernel, size_t bytes);
 
 // 128-bit streaming load: read-only path, do not allocate in L1 (each byte is used once).
 __device__ __forceinline__ uint4 ld_stream_u4(const void* p) {

@@ -60,15 +60,15 @@ def _assert_spans_exceed(what, n, per_frame, per_cta, warps, limit):
 
 
 def _csa_premise(n, nbytes):
-    # csa::launch (hist_csa.cuh:233-239): blocks_per_frame = nbytes / kWarpBlock, ctas = ceil(total / (kWarps * 4))
-    # capped at sm_count(); hist16_csa_kernel (hist_csa.cuh:158-168) splits total_blocks evenly over the warps
+    # csa::launch in hist_csa.cuh: blocks_per_frame = nbytes / kWarpBlock, ctas = ceil(total / (kWarps * 4)) capped
+    # at sm_count(); hist16_csa_kernel splits total_blocks evenly over the warps
     assert nbytes >= 8 * CSA_BLOCK
     _assert_spans_exceed("hist16_csa_kernel", n, nbytes // CSA_BLOCK, CSA_WARPS * 4, CSA_WARPS, CSA_MAX_BLOCKS)
 
 
 def _nvs_premise(n, h, w, pitch):
-    # nvs::eligible (nv12_stream.cuh:382-388); nvs::launch (nv12_stream.cuh:409-416): steps_per_frame =
-    # ceil(width / 16 * height / 2 / 32), ctas = ceil(total / (kWarps * 8)) capped at sm_count()
+    # nvs::eligible and nvs::launch in nv12_stream.cuh: steps_per_frame = ceil(width / 16 * height / 2 / 32),
+    # ctas = ceil(total / (kWarps * 8)) capped at sm_count()
     assert w % 16 == 0 and pitch % 16 == 0 and h % 2 == 0 and w * h >= 64 * 1024
     spf = -(-(w // 16 * (h // 2)) // 32)
     _assert_spans_exceed("nv12_stream_kernel", n, spf, NVS_WARPS * 8, NVS_WARPS, NVS_MAX_STEPS)
