@@ -173,7 +173,18 @@ SCN_API int scn_convert_color_nv12(const uint8_t* const* host_luma_ptrs, const u
  *   polySigma, flags=0)->calc; the reference constructs it with (3, 0.5, 15, 3, 5, 1.2), :68-69)
  * For each of n frame pairs writes a dense flow field float32[H][W][2] (dx, dy) to
  * host_flow_ptrs[i].  Floating point: matches cv2.calcOpticalFlowFarneback within a tolerance
- * (max |d| <= 2e-3 px on well-conditioned input; see tests/test_flow_gpu.py), not bit-exact.
+ * (max |d| <= 2e-3 px, mean <= 1e-4 px on well-conditioned input), not bit-exact.  That holds over the
+ * supported range, not only at the reference's arguments: tests/test_flow_params_gpu.py checks it for
+ * num_levels 0-8, pyr_scale 0.3-0.8, win_size 2-21, num_iters 1-6, poly_n 1-7 and frames from 1 x 1 up.
+ * Two kinds of pixel can lie further off: windows too small to condition the 2x2 solve (win_size 2), and
+ * a pixel whose warped position lands within float rounding of the frame edge, where UpdateMatrices
+ * switches branch (one window footprint in that test's 1080p case).
+ * Supported: win_size >= 2, 1 <= poly_n <= 7, poly_sigma > 0, 0 <= num_levels <= 15,
+ * 0 < pyr_scale < 1, num_iters >= 1.  Anything else returns SCN_E_BADARG.  win_size 1 is refused
+ * because OpenCV's window-sum code does not compute a 1 x 1 box there, so no result could match cv2.
+ * A pyramid level whose Gaussian needs more than 65 taps returns SCN_E_UNSUPPORTED before any launch
+ * (ksize = max(3, lrint(5 sigma) | 1) with sigma = (1 / pyr_scale^k - 1) / 2: num_levels <= 4 at
+ * pyr_scale 0.5; levels that the 32-pixel minimum cuts off do not count).
  * `workspace` is caller-owned device scratch of scn_farneback_workspace_bytes(w, h) bytes,
  * reusable across calls on the same stream.
  */

@@ -307,18 +307,20 @@ static void orc_gauss_kernel(int ksize, double sigma, float* k) {
   }
   if (sigma <= 0) sigma = ((ksize - 1) * 0.5 - 1) * 0.3 + 0.8;
   double scale2x = -0.5 / (sigma * sigma), sum = 0;
-  double tmp[64];
+  double* tmp = (double*)malloc(sizeof(double) * (size_t)ksize);
   for (int i = 0; i < ksize; ++i) {
     double x = i - (ksize - 1) * 0.5;
     tmp[i] = exp(scale2x * x * x);
     sum += tmp[i];
   }
   for (int i = 0; i < ksize; ++i) k[i] = (float)(tmp[i] / sum);
+  free(tmp);
 }
 
 /* GaussianBlur on float, separable, BORDER_REFLECT_101 (OpenCV default) */
+/* (ksize grows with the pyramid depth: 79 taps at level 5 of pyr_scale 0.5, so the taps are sized to it) */
 static void orc_gaussian_blur_f32(const float* src, int w, int h, int ksize, double sigma, float* dst) {
-  float k[64];
+  float* k = (float*)malloc(sizeof(float) * (size_t)ksize);
   orc_gauss_kernel(ksize, sigma, k);
   int r = ksize / 2;
   float* tmp = (float*)malloc(sizeof(float) * (size_t)w * h);
@@ -335,6 +337,7 @@ static void orc_gaussian_blur_f32(const float* src, int w, int h, int ksize, dou
       dst[(size_t)y * w + x] = s;
     }
   free(tmp);
+  free(k);
 }
 
 /* cv::resize INTER_LINEAR for float images, cn channels (half-pixel centres, edge clamp) */

@@ -733,8 +733,10 @@ extern "C" int scn_farneback_u8c3_chain(const uint8_t* const* host_prev_ptrs, co
                                         void* stream) {
   using namespace scn;
   if (chain && (*chain < 0 || *chain > 2)) return SCN_E_BADARG;
+  // win_size 1 is refused: at window half-width 0 OpenCV's FarnebackUpdateFlow_Blur does not compute a 1 x 1 box
+  // (its running sums appear to start one row too many), so the plain box here would not match cv2 there
   if (n < 0 || width <= 0 || height <= 0 || num_levels < 0 || num_levels > 15 || pyr_scale <= 0 || pyr_scale >= 1 ||
-      win_size < 1 || num_iters < 1 || poly_n < 1 || poly_n > kMaxPolyN || poly_sigma <= 0)
+      win_size < 2 || num_iters < 1 || poly_n < 1 || poly_n > kMaxPolyN || poly_sigma <= 0)
     return SCN_E_BADARG;
   if (n == 0) return 0;
   if (!host_prev_ptrs || !host_next_ptrs || !host_flow_ptrs || !workspace) return SCN_E_BADARG;
