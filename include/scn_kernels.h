@@ -8,7 +8,8 @@
  *
  * Conventions
  *   - `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).  Every call
- *     only ENQUEUES work on that stream and returns; nothing synchronises, nothing allocates.
+ *     only ENQUEUES work on that stream and returns; nothing synchronises, nothing allocates
+ *     (except scn_jpeg_encode_u8, whose output size depends on the data: see there).
  *   - Pointers are DEVICE pointers on the current CUDA device unless the parameter name
  *     starts with `host_`.  `host_*_ptrs` arrays are read synchronously during the call
  *     (they are copied into the kernel's launch parameters) and may be freed on return.
@@ -165,6 +166,32 @@ SCN_API int scn_convert_color_u8(const uint8_t* const* host_src_ptrs, int n, int
 SCN_API int scn_convert_color_nv12(const uint8_t* const* host_luma_ptrs, const uint8_t* const* host_chroma_ptrs,
                                    size_t pitch, int n, int width, int height, int code,
                                    uint8_t* const* host_dst_ptrs, void* stream);
+
+/* ---------------------------------------------------------------------------------------
+ * JPEG  (the GPU kernel of the ImageEncoder op with format "jpg": upstream, scannertools encoded
+ *        with cv::imencode(".jpg")).  Byte for byte what cv2.imencode('.jpg', frame, [IMWRITE_JPEG_QUALITY,
+ *        quality]) writes with cv2's libjpeg defaults: baseline JFIF, 4:2:0 for three channels, Annex K
+ *        Huffman tables, no restart markers.
+ * scn_jpeg_encode_u8: n dense u8 frames of one geometry, `channels` 3 (RGB, as the pipeline stores them;
+ *   cv2 would be given the BGR frame) or 1 (gray), any base alignment -> n complete JFIF files.  Quality
+ *   1-100.  Pointer list; batches over 64 frames are split into launches.
+ *   Unlike the rest of this header the call synchronises `stream` twice (it reads back each frame's bit count
+ *   to size its scratch, then each frame's 0xFF count to size the output) and allocates its device scratch
+ *   from a stream-ordered pool the library keeps per device.  When the sizes are known it calls
+ *   alloc_out(alloc_ctx, total) once for a device buffer of `total` bytes, writes host_sizes[0..n), and
+ *   enqueues the files into that buffer back to back (file i at the sum of the sizes before it); they are
+ *   ready in stream order when the call returns.  A null alloc_out result returns SCN_E_ALLOC.
+ *   channels other than 1 and 3, or a side over 65,500 (libjpeg's JPEG_MAX_DIMENSION): SCN_E_UNSUPPORTED.
+ * scn_jpeg_encode_bound: bytes no file of that geometry exceeds at any quality (0 for an unsupported
+ *   geometry): the header, every block at its longest code (26 bits per AC coefficient, 22 for the DC),
+ *   every byte stuffed, and the EOI.
+ */
+#define SCN_E_ALLOC (-4)
+typedef void* (*scn_alloc_fn)(void* ctx, size_t bytes);
+SCN_API size_t scn_jpeg_encode_bound(int width, int height, int channels);
+SCN_API int scn_jpeg_encode_u8(const uint8_t* const* host_src_ptrs, int n, int width, int height, int channels,
+                               int quality, scn_alloc_fn alloc_out, void* alloc_ctx, size_t* host_sizes,
+                               void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * OpticalFlow  (replaces OpticalFlowKernelCPU::execute, tests/test_ops.cpp:79-98:

@@ -13,6 +13,8 @@ LIB_PATH = os.environ.get("SCN_KERNELS_LIB") or os.path.join(_HERE, "lib", "libs
 _c = ctypes
 _VP = _c.c_void_p
 _PP = _c.POINTER(_c.c_void_p)
+# scn_alloc_fn: (ctx, bytes) -> device pointer
+ALLOC_FN = _c.CFUNCTYPE(_c.c_void_p, _c.c_void_p, _c.c_size_t)
 
 # name -> (restype, argtypes); must list every symbol declared in include/scn_kernels.h
 SIGNATURES = {
@@ -47,6 +49,9 @@ SIGNATURES = {
     "scn_convert_color_u8": (_c.c_int, [_PP, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _PP, _VP]),
     "scn_convert_color_nv12": (_c.c_int, [_PP, _PP, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _PP,
                                           _VP]),
+    "scn_jpeg_encode_bound": (_c.c_size_t, [_c.c_int, _c.c_int, _c.c_int]),
+    "scn_jpeg_encode_u8": (_c.c_int, [_PP, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int, ALLOC_FN, _VP,
+                                      _c.POINTER(_c.c_size_t), _VP]),
 }
 
 _lib = None

@@ -4,6 +4,10 @@
 //                 of type "Image", ImageEncoderArgs{format}.  The reference compresses with lodepng;
 //                 here the stream is written with zlib (deflate) and the standard minimum-sum filter
 //                 heuristic -- the file bytes differ, the decoded pixels are identical (lossless).
+//                 The GPU kernel of the op also writes JPEG (format "jpg"): scannertools encoded with
+//                 cv::imencode, and scn_jpeg_encode_u8 gives cv2.imencode's bytes exactly (HWC u8 frames with
+//                 1 or 3 channels, ImageEncoderArgs.quality, 95 when 0).  "png" on the GPU kernel copies the
+//                 frames to the host and writes the same PNG as the CPU kernel.
 //   ImageDecoder  PNG bytes -> frame (the op pipelines pair with it: examples/tutorials/
 //                 05_sources_sinks.py:41-47; upstream it lives in scannertools and calls
 //                 cv::imdecode).  Non-interlaced PNG of colour types 0, 2, 4, 6 with 8 or 16 bits.
@@ -22,6 +26,7 @@
 #include "scanner/api/kernel.h"
 #include "scanner/api/op.h"
 #include "scanner/util/memory.h"
+#include "scn_kernels.h"
 #include "stdlib_args.pb.h"
 
 namespace scanner {
@@ -235,6 +240,141 @@ class ImageEncoderKernel : public BatchedKernel {
 
 REGISTER_OP(ImageEncoder).frame_input("frame").output("img", ColumnType::Bytes, "Image").protobuf_name("ImageEncoderArgs");
 REGISTER_KERNEL(ImageEncoder, ImageEncoderKernel).device(DeviceType::CPU).batch(8).num_devices(1);
+
+// ---- GPU kernel: JPEG from sm_90a kernels (scn_jpeg_encode_u8), the encoded bytes delivered on the host -----
+class ImageEncoderKernelGPU : public BatchedKernel {
+ public:
+  ImageEncoderKernelGPU(const KernelConfig& config) : BatchedKernel(config), device_(config.devices[0]) {
+    ImageEncoderArgs args;
+    if (!args.ParseFromArray(config.args.data(), (int)config.args.size())) {
+      RESULT_ERROR(&valid_, "Could not parse ImageEncoderArgs");
+      return;
+    }
+    const std::string fmt = args.format().empty() ? "png" : args.format();
+    if (fmt == "png" || fmt == "PNG") {
+      jpeg_ = false;
+    } else if (fmt == "jpg" || fmt == "jpeg" || fmt == "JPEG") {
+      jpeg_ = true;
+    } else {
+      RESULT_ERROR(&valid_, "Invalid format type specified to ImageEncoder: %s. Valid types are: png, jpg.",
+                   fmt.c_str());
+      return;
+    }
+    quality_ = args.quality() == 0 ? 95 : args.quality();
+    if (quality_ < 1 || quality_ > 100) {
+      RESULT_ERROR(&valid_, "ImageEncoder quality %d is outside [1, 100]", quality_);
+      return;
+    }
+    valid_.set_success(true);
+  }
+  void validate(Result* result) override { result->CopyFrom(valid_); }
+
+  void execute(const BatchedElements& in, BatchedElements& out) override {
+    const Elements& frames = in[0];
+    if (frames.empty()) return;
+    if (cudaSetDevice(device_.id) != cudaSuccess) LOG(FATAL) << "ImageEncoder: cannot select GPU " << device_.id;
+    if (!jpeg_) {
+      for (const Element& e : frames) encode_png_row(e, out[0]);
+      return;
+    }
+    // runs of equal geometry, one scn_jpeg_encode_u8 call each
+    size_t i = 0;
+    while (i < frames.size()) {
+      size_t j = i + 1;
+      if (!frames[i].is_null())
+        while (j < frames.size() && !frames[j].is_null() &&
+               frames[j].as_const_frame()->as_frame_info() == frames[i].as_const_frame()->as_frame_info())
+          ++j;
+      encode_jpeg_run(frames, i, j, out[0]);
+      i = j;
+    }
+  }
+
+ private:
+  static std::string unsupported(const Frame* f) {
+    if (f->layout != FrameLayout::HWC) return "JPEG needs HWC frames, got an NV12 element";
+    if ((proto::FrameType)f->type != proto::U8)
+      return "JPEG needs uint8 frames, got type " + std::to_string((int)(proto::FrameType)f->type);
+    if (f->channels() != 1 && f->channels() != 3)
+      return "JPEG needs 1- or 3-channel frames, got " + std::to_string(f->channels()) + " channels";
+    if (f->width() > 65500 || f->height() > 65500)
+      return "JPEG frames are at most 65500 x 65500, got " + std::to_string(f->width()) + " x " +
+             std::to_string(f->height());
+    return "";
+  }
+
+  void encode_png_row(const Element& e, Elements& col) {
+    std::string err = e.is_null() ? std::string("null frame") : "";
+    std::vector<u8> png;
+    if (err.empty()) {
+      const Frame* f = e.as_const_frame();
+      Frame* host = new_frame(CPU_DEVICE, f->as_frame_info());
+      memcpy_buffer(host->data, CPU_DEVICE, f->data, device_, f->size());
+      err = encode_png(host, png);
+      delete_buffer(CPU_DEVICE, host->data);
+      delete host;
+    }
+    if (!err.empty()) {
+      report_kernel_error("ImageEncoder, row " + std::to_string(e.index) + ": " + err);
+      col.push_back(Element());
+      return;
+    }
+    u8* buf = new_buffer(CPU_DEVICE, png.size());
+    memcpy(buf, png.data(), png.size());
+    insert_element(col, buf, png.size());
+  }
+
+  static void* alloc_on(void* ctx, size_t bytes) {
+    auto* self = static_cast<ImageEncoderKernelGPU*>(ctx);
+    self->staging_ = new_buffer(self->device_, bytes ? bytes : 1);
+    return self->staging_;
+  }
+
+  void encode_jpeg_run(const Elements& frames, size_t i0, size_t i1, Elements& col) {
+    const size_t n = i1 - i0;
+    const Frame* f0 = frames[i0].is_null() ? nullptr : frames[i0].as_const_frame();
+    const std::string why = f0 ? unsupported(f0) : std::string("null frame");
+    if (!why.empty()) {
+      report_kernel_error("ImageEncoder, row " + std::to_string(frames[i0].index) + ": " + why);
+      for (size_t k = 0; k < n; ++k) col.push_back(Element());
+      return;
+    }
+    std::vector<const u8*> src;
+    for (size_t k = i0; k < i1; ++k) src.push_back(frames[k].as_const_frame()->data);
+    std::vector<size_t> sizes(n);
+    staging_ = nullptr;
+    cudaStream_t stream = (cudaStream_t)device_stream(device_);
+    const int rc = scn_jpeg_encode_u8(src.data(), (int)n, f0->width(), f0->height(), f0->channels(), quality_,
+                                      &ImageEncoderKernelGPU::alloc_on, this, sizes.data(), stream);
+    if (rc != 0) LOG(FATAL) << "scn_jpeg_encode_u8 failed with code " << rc;
+    // one copy of the packed files to the host, in the synchronisation the encoder needs anyway
+    u8* block = new_block_buffer_sizes(CPU_DEVICE, sizes);
+    size_t total = 0;
+    for (size_t s : sizes) total += s;
+    if (cudaMemcpyAsync(block, staging_, total, cudaMemcpyDeviceToHost, stream) != cudaSuccess ||
+        cudaStreamSynchronize(stream) != cudaSuccess)
+      LOG(FATAL) << "ImageEncoder: copying encoded JPEG files from GPU " << device_.id << " failed";
+    delete_buffer(device_, staging_);
+    staging_ = nullptr;
+    size_t at = 0;
+    for (size_t k = 0; k < n; ++k) {
+      insert_element(col, block + at, sizes[k]);
+      at += sizes[k];
+    }
+  }
+
+  DeviceHandle device_;
+  bool jpeg_ = false;
+  int quality_ = 95;
+  u8* staging_ = nullptr;  // the device buffer scn_jpeg_encode_u8 writes the files of one run into
+  Result valid_;
+};
+
+REGISTER_KERNEL(ImageEncoder, ImageEncoderKernelGPU)
+    .device(DeviceType::GPU)
+    .batch(64)
+    .num_devices(1)
+    .output_device("img", DeviceType::CPU);
 
 class ImageDecoderKernel : public BatchedKernel {
  public:

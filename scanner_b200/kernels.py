@@ -219,6 +219,62 @@ def convert_color(frames, code, width=None, height=None):
     return outs
 
 
+def jpeg_encode_bound(width, height, channels=3):
+    """Bytes no JPEG file of that geometry exceeds at any quality (scn_jpeg_encode_bound)."""
+    return cabi.lib().scn_jpeg_encode_bound(width, height, channels)
+
+
+def jpeg_encode(frames, quality=95):
+    """Baseline JPEG files of uint8 frames, byte for byte cv2.imencode('.jpg', bgr, [cv2.IMWRITE_JPEG_QUALITY,
+    quality]) with bgr the frame's channels reversed (frames are RGB) or the gray frame itself.
+
+    frames: (N,H,W,C) uint8 CUDA tensor or a list of (H,W,C) tensors, shapes may differ (one call per run of
+    equal shape); C is 3 or 1, and a frame need not be aligned.  -> list of N bytes objects.  Synchronises
+    the current stream."""
+    L = cabi.lib()
+
+    def run(src_ptrs, h, w, c, device):
+        keep = []
+
+        def alloc(_ctx, nbytes):
+            keep.append(torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device))
+            return keep[-1].data_ptr()
+
+        cb = cabi.ALLOC_FN(alloc)
+        sizes = (ctypes.c_size_t * len(src_ptrs))()
+        sp, k1 = cabi.ptr_array(src_ptrs)
+        rc = L.scn_jpeg_encode_u8(sp, len(src_ptrs), w, h, c, int(quality), cb, None, sizes, _stream())
+        cabi.check(rc, "scn_jpeg_encode_u8")
+        data = keep[0].cpu().numpy().tobytes()  # on the current stream, after the files are written
+        out, at = [], 0
+        for s in sizes:
+            out.append(data[at:at + s])
+            at += s
+        return out
+
+    if isinstance(frames, torch.Tensor):
+        _need_cuda(frames)
+        assert frames.dtype == torch.uint8 and frames.dim() == 4
+        frames = frames.contiguous()
+        n, h, w, c = frames.shape
+        if n == 0:
+            return []
+        return run([frames.data_ptr() + i * h * w * c for i in range(n)], h, w, c, frames.device)
+    lst = [t.contiguous() for t in frames]
+    _need_cuda(*lst)
+    for t in lst:
+        assert t.dtype == torch.uint8 and t.dim() == 3
+    outs = []
+    i = 0
+    while i < len(lst):
+        j = i + 1
+        while j < len(lst) and lst[j].shape == lst[i].shape:
+            j += 1
+        outs += run([t.data_ptr() for t in lst[i:j]], *lst[i].shape, lst[i].device)
+        i = j
+    return outs
+
+
 def optical_flow_sequence(frames, workspace=None, pairs_per_call=None):
     """Flow of every consecutive pair of a clip: (N,H,W,3) uint8 -> (N-1,H,W,2) float32.  Every frame is expanded
     once (scn_farneback_u8c3_chain); pairs_per_call splits the clip over several calls on one workspace, the way
