@@ -79,7 +79,8 @@ SCN_API int scn_hist16_u8c3_strided(const uint8_t* base, size_t stride_bytes, in
  *
  * A "plan" is the per-(src size, dst size) coefficient table (x/y tap offsets and 11-bit
  * weights).  The caller owns its storage: ask for the size, fill it on the host, copy it to the
- * device once, pass the device copy to every launch with those sizes.
+ * device once, pass the device copy to every launch with those sizes.  A destination of more
+ * than INT_MAX pixels returns SCN_E_BADARG (here and in scn_nv12_hist_resize) before any launch.
  */
 SCN_API void scn_resize_target(int src_w, int src_h, int arg_w, int arg_h, int arg_min,
                        int arg_preserve_aspect, int* out_w, int* out_h);

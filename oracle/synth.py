@@ -22,6 +22,30 @@ def frame(seed, h, w, kind):
     return rand_frame(seed, h, w) if kind == 0 else smooth_frame(seed, h, w)
 
 
+# Sides at which a Resize table changes behaviour: 1 px (both taps clamp), small integer factors, powers of two and
+# their neighbours, the 224 model input, video heights and widths.
+RESIZE_SIDES = (1, 2, 3, 4, 5, 7, 8, 15, 16, 17, 31, 33, 63, 64, 65, 100, 223, 224, 225, 479, 480, 1079, 1080, 1920)
+
+
+def resize_geometries(seed, n, sides=RESIZE_SIDES):
+    """n seeded (src_w, src_h, dst_w, dst_h), every side drawn from `sides`.  Every 10th geometry is an exact 2x
+    downscale on both axes (the INTER_AREA re-route) and every 10th + 5 on the width only (which stays linear)."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for i in range(n):
+        sw, sh, dw, dh = (int(x) for x in rng.choice(sides, 4))
+        if i % 10 == 0:
+            dw, dh = (int(x) for x in rng.choice([s for s in sides if 2 * s <= max(sides)], 2))
+            sw, sh = 2 * dw, 2 * dh
+        elif i % 10 == 5:
+            dw = int(rng.choice([s for s in sides if 2 * s <= max(sides)]))
+            sw = 2 * dw
+            if sh == 2 * dh:
+                dh = sh
+        out.append((sw, sh, dw, dh))
+    return out
+
+
 def nv12_surface(seed, h, w, pitch=None):
     pitch = pitch or w
     rng = np.random.default_rng(seed)

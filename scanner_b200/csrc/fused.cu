@@ -4,6 +4,8 @@
 // read them back).  Here the surface (1.5 WH bytes) is the only large read: the histogram is
 // taken from RGB values converted in registers, and the resize converts just the 4 taps of each
 // destination pixel.  Results are bit-identical to the three-pass composition.
+#include <limits.h>
+
 #include "nv12_stream.cuh"
 
 #include "nv12_math.cuh"
@@ -176,7 +178,8 @@ extern "C" int scn_nv12_hist_resize(const uint8_t* const* host_luma_ptrs,
   const bool do_resize = host_dst_ptrs != nullptr;
   if (!do_hist && !do_resize) return SCN_E_BADARG;
   const bool area2x = do_resize && (width == 2 * dst_w && height == 2 * dst_h);
-  if (do_resize && (dst_w <= 0 || dst_h <= 0)) return SCN_E_BADARG;
+  // nv12_resize_kernel indexes destination pixels with an int
+  if (do_resize && (dst_w <= 0 || dst_h <= 0 || (int64_t)dst_w * dst_h > INT_MAX)) return SCN_E_BADARG;
   if (do_resize && !area2x && !plan) return SCN_E_PLAN;
   cudaStream_t st = (cudaStream_t)stream;
   if (do_hist) {
@@ -219,7 +222,7 @@ extern "C" int scn_nv12_hist_resize(const uint8_t* const* host_luma_ptrs,
       if (hrc || !do_resize) return hrc;
     }
     const MutPtrBatch d = gather<MutPtrBatch>(host_dst_ptrs, i0, cnt);
-    dim3 g2((unsigned)((dst_w * dst_h + 255) / 256), (unsigned)cnt);
+    dim3 g2((unsigned)(((int64_t)dst_w * dst_h + 255) / 256), (unsigned)cnt);
     return launch_kernel("nv12_resize_kernel", rst, [&] {
       nv12_resize_kernel<<<g2, 256, 0, rst>>>(l, c, pitch, width, height, d, (const uint8_t*)plan, dst_w, dst_h,
                                             area2x ? 1 : 0);

@@ -3,7 +3,9 @@
 // (tests/test_ops.cpp:13-59 Histogram, :114-170 Resize, :239-310 Blur) -- but the kernels are
 // registered for DeviceType::GPU and run the sm_90a kernels of libscn_kernels.so on the
 // pipeline instance's stream.  Loaded with dlopen like any user op library (Client.load_op).
+#include <climits>
 #include <map>
+#include <string>
 
 #include "scanner/api/kernel.h"
 #include "scanner/api/op.h"
@@ -40,15 +42,22 @@ bool is_nv12(const Frame* f) { return f->layout == FrameLayout::NV12; }
 int pic_width(const Frame* f) { return f->width(); }
 int pic_height(const Frame* f) { return is_nv12(f) ? f->height() / 3 * 2 : f->height(); }
 
-void require_rgb8(const Frame* f, const char* op) {
+// why a frame element is neither an HxWx3 uint8 frame nor a well-formed NV12 element; empty when it is one
+std::string rgb8_problem(const Frame* f) {
   if (is_nv12(f)) {
     if (f->channels() != 1 || (proto::FrameType)f->type != proto::U8 || f->height() % 3 != 0 || (f->width() & 1))
-      LOG(FATAL) << op << ": malformed NV12 frame element " << f->height() << "x" << f->width();
-    return;
+      return "malformed NV12 frame element " + std::to_string(f->height()) + "x" + std::to_string(f->width());
+    return "";
   }
   if (f->channels() != 3 || (proto::FrameType)f->type != proto::U8)
-    LOG(FATAL) << op << " expects HxWx3 uint8 frames, got " << f->height() << "x" << f->width() << "x"
-               << f->channels() << " type " << (int)(proto::FrameType)f->type;
+    return "expects HxWx3 uint8 frames, got " + std::to_string(f->height()) + "x" + std::to_string(f->width()) + "x" +
+           std::to_string(f->channels()) + " type " + std::to_string((int)(proto::FrameType)f->type);
+  return "";
+}
+
+void require_rgb8(const Frame* f, const char* op) {
+  const std::string why = rgb8_problem(f);
+  if (!why.empty()) LOG(FATAL) << op << ": " << why;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -103,19 +112,32 @@ class ResizeKernelGPU : public BatchedKernel {
     for (auto& kv : plans_) delete_buffer(device_, kv.second);
   }
 
-  void new_stream(const std::vector<u8>& args) override { args_.ParseFromArray(args.data(), (int)args.size()); }
+  // a parse failure is reported by execute(), where the failing row is known
+  void new_stream(const std::vector<u8>& args) override {
+    args_ = ResizeArgs();
+    args_ok_ = args_.ParseFromArray(args.data(), (int)args.size());
+  }
 
   void execute(const BatchedElements& input_columns, BatchedElements& output_columns) override {
     const Elements& frames = input_columns[0];
     if (frames.empty()) return;
     CU_CHECK(cudaSetDevice(device_.id));
     for_each_run(frames, [&](size_t i0, size_t i1, const Frame* f0) {
-      require_rgb8(f0, "Resize");
+      const i32 n = (i32)(i1 - i0);
       const int sw = pic_width(f0), sh = pic_height(f0);
       int tw = 0, th = 0;
-      scn_resize_target(sw, sh, args_.width(), args_.height(), args_.min(), args_.preserve_aspect(), &tw, &th);
-      if (tw <= 0 || th <= 0) LOG(FATAL) << "Resize: invalid target size " << tw << "x" << th;
-      const i32 n = (i32)(i1 - i0);
+      std::string why = args_ok_ ? rgb8_problem(f0) : "could not parse ResizeArgs";
+      if (why.empty()) {
+        scn_resize_target(sw, sh, args_.width(), args_.height(), args_.min(), args_.preserve_aspect(), &tw, &th);
+        if (tw <= 0 || th <= 0 || (int64_t)tw * th > INT_MAX)
+          why = "invalid target size " + std::to_string(tw) + "x" + std::to_string(th) + " for a " +
+                std::to_string(sw) + "x" + std::to_string(sh) + " frame";
+      }
+      if (!why.empty()) {
+        report_kernel_error("Resize, row " + std::to_string(frames[i0].index) + ": " + why);
+        for (i32 i = 0; i < n; ++i) output_columns[0].push_back(Element());
+        return;
+      }
       FrameInfo info(th, tw, 3, FrameType::U8);
       std::vector<Frame*> outs = new_frames(device_, info, n);
       std::vector<const u8*> src;
@@ -154,6 +176,7 @@ class ResizeKernelGPU : public BatchedKernel {
 
   DeviceHandle device_;
   ResizeArgs args_;
+  bool args_ok_ = true;
   std::map<std::array<int, 4>, u8*> plans_;
 };
 

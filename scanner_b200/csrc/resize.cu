@@ -6,6 +6,7 @@
 //   exact 2x downscale in both axes is re-routed to the 2x2 box average (INTER_AREA fast path).
 // The coefficient tables ("plan") are computed on the host with the same float expressions
 // OpenCV uses and handed to the kernel, so host and device cannot round differently.
+#include <limits.h>
 #include <math.h>
 #include <string.h>
 
@@ -88,6 +89,8 @@ resize_area2x_kernel(PtrBatch src, MutPtrBatch dst, int sw, int dw, int dh) {
 int launch_resize(const uint8_t* const* sp, int n, int sw, int sh, uint8_t* const* dp, int dw,
                   int dh, const void* plan, cudaStream_t st) {
   if (n < 0 || sw <= 0 || sh <= 0 || dw <= 0 || dh <= 0) return SCN_E_BADARG;
+  // the kernels index destination pixels with an int
+  if ((int64_t)dw * dh > INT_MAX) return SCN_E_BADARG;
   if (n == 0) return 0;
   if (!sp || !dp) return SCN_E_BADARG;
   const bool area2x = (sw == 2 * dw && sh == 2 * dh);
@@ -95,7 +98,7 @@ int launch_resize(const uint8_t* const* sp, int n, int sw, int sh, uint8_t* cons
   return for_each_chunk(n, [&](int i0, int cnt) {
     const PtrBatch s = gather<PtrBatch>(sp, i0, cnt);
     const MutPtrBatch d = gather<MutPtrBatch>(dp, i0, cnt);
-    dim3 grid((unsigned)((dw * dh + 255) / 256), (unsigned)cnt);
+    dim3 grid((unsigned)(((int64_t)dw * dh + 255) / 256), (unsigned)cnt);
     if (area2x)
       return launch_kernel("resize_area2x_kernel", st,
                            [&] { resize_area2x_kernel<<<grid, 256, 0, st>>>(s, d, sw, dw, dh); });

@@ -38,13 +38,23 @@ def test_abi_version_and_launch_counter():
 
 def test_resize_target_matches_oracle():
     l = cabi.lib()
-    for (sw, sh, w, h, mn, pa) in [(1920, 1080, 224, 224, 0, 0), (1920, 1080, 0, 540, 0, 1),
-                                   (1920, 1080, 640, 0, 0, 1), (640, 480, 1000, 1000, 1, 0),
-                                   (640, 480, 320, 1000, 1, 0), (640, 480, 0, 0, 0, 0),
-                                   (33, 77, 100, 0, 1, 1)]:
+    fixed = [(1920, 1080, 224, 224, 0, 0), (1920, 1080, 0, 540, 0, 1), (1920, 1080, 640, 0, 0, 1),
+             (640, 480, 1000, 1000, 1, 0), (640, 480, 320, 1000, 1, 0), (640, 480, 0, 0, 0, 0), (33, 77, 100, 0, 1, 1),
+             (1920, 1080, 1, 0, 0, 1), (1920, 1080, 0, 0, 0, 1), (1080, 1920, 0, 1, 0, 1)]
+    rng = np.random.default_rng(17)
+    sides = (0,) + synth.RESIZE_SIDES
+    sweep = [tuple(int(x) for x in rng.choice(sides, 4)) + (int(rng.integers(2)), int(rng.integers(2)))
+             for _ in range(3000)]
+    zero = 0
+    for (sw, sh, w, h, mn, pa) in fixed + [g for g in sweep if g[0] and g[1]]:
         ow, oh = ctypes.c_int(), ctypes.c_int()
         l.scn_resize_target(sw, sh, w, h, mn, pa, ctypes.byref(ow), ctypes.byref(oh))
-        assert (ow.value, oh.value) == oracle.resize_target(sw, sh, w, h, bool(mn), bool(pa))
+        assert (ow.value, oh.value) == oracle.resize_target(sw, sh, w, h, bool(mn), bool(pa)), (sw, sh, w, h, mn, pa)
+        zero += ow.value <= 0 or oh.value <= 0
+    # the zero targets the Resize op refuses: 1920 x 1080 at width 1 with preserve_aspect is 1 x 0
+    assert oracle.resize_target(1920, 1080, 1, 0, preserve_aspect=True) == (1, 0)
+    assert oracle.resize_target(1920, 1080, 0, 0, preserve_aspect=True) == (0, 0)
+    assert zero > 100
 
 
 def _apply_plan_numpy(img, plan_bytes, dw, dh):
@@ -71,6 +81,48 @@ def test_resize_plan_matches_oracle(h, w, dh, dw):
     assert l.scn_resize_plan_fill(w, h, dw, dh, buf.ctypes.data) == 0
     img = synth.rand_frame(7, h, w)
     assert (_apply_plan_numpy(img, buf, dw, dh) == oracle.resize(img, dw, dh)).all()
+
+
+def _cv2_taps(ssz, dsz, clamp_x):
+    """cv::resize's INTER_LINEAR table for one axis restated in float32 numpy (OpenCV imgproc/src/resize.cpp):
+    f = (float)((d + 0.5) * scale - 0.5), s = floor(f), weights saturate_cast<short>((1 - f, f) * 2048).  On x a tap
+    left of 0 or at/after the last pixel becomes (edge, weight 2048, 0); on y the weights stay and the rows clamp."""
+    scale = 1.0 / (dsz / ssz)
+    f = ((np.arange(dsz) + 0.5) * scale - 0.5).astype(np.float32)
+    s = np.floor(f).astype(np.int64)
+    f = f - s.astype(np.float32)
+    if clamp_x:
+        f[s < 0], s[s < 0] = 0, 0
+        last = s >= ssz - 1
+        f[last], s[last] = 0, ssz - 1
+    w0 = np.rint((np.float32(1) - f) * np.float32(2048)).astype(np.int64)
+    w1 = np.rint(f * np.float32(2048)).astype(np.int64)
+    return np.stack([np.clip(s, 0, ssz - 1), np.clip(s + 1, 0, ssz - 1), w0, w1], 1)
+
+
+def test_resize_plan_equals_cv2_over_a_sweep():
+    """The product's plan over ~2000 seeded geometries (every side from synth.RESIZE_SIDES): the header, every tap
+    and weight against cv2's table, and the plan applied with numpy against live cv2.resize.  Exact-2x geometries
+    take INTER_AREA in cv2 and in the kernels, so there only the header flag and the table are checked."""
+    cv2 = pytest.importorskip("cv2")
+    l = cabi.lib()
+    big = synth.rand_frame(23, 1920, 1920)
+    area = 0
+    for k, (sw, sh, dw, dh) in enumerate(synth.resize_geometries(5, 2000)):
+        buf = np.zeros(l.scn_resize_plan_bytes(dw, dh), np.uint8)
+        assert l.scn_resize_plan_fill(sw, sh, dw, dh, buf.ctypes.data) == 0
+        hdr, taps = buf.view(np.int32)[:8], buf.view(np.int32)[8:].reshape(-1, 4)
+        area2x = sw == 2 * dw and sh == 2 * dh
+        assert list(hdr[1:6]) == [sw, sh, dw, dh, int(area2x)], (sw, sh, dw, dh)
+        assert (taps[:dw] == _cv2_taps(sw, dw, True)).all(), ("x", sw, sh, dw, dh)
+        assert (taps[dw:] == _cv2_taps(sh, dh, False)).all(), ("y", sw, sh, dw, dh)
+        area += area2x
+        if area2x:
+            continue
+        img = big[:sh, :sw] if k % 2 else np.full((sh, sw, 3), 255 * (k % 4 == 0), np.uint8)
+        want = cv2.resize(img, (dw, dh), interpolation=cv2.INTER_LINEAR)
+        assert (_apply_plan_numpy(img, buf, dw, dh) == want).all(), (sw, sh, dw, dh)
+    assert area >= 200
 
 
 def test_bad_arguments_are_rejected_without_a_gpu():

@@ -76,6 +76,18 @@ def test_nv12_exhaustive_yuv_triples():
         assert (rgb[..., 0] == r).all()
 
 
+def test_resize_equals_live_cv2_over_a_sweep():
+    """oracle.resize against cv2.resize itself on the ~2000 seeded geometries test_cabi_host.py holds the product's
+    plan to, random and constant 0 / 255 frames."""
+    import pytest
+    cv2 = pytest.importorskip("cv2")
+    big = synth.rand_frame(23, 1920, 1920)
+    for k, (sw, sh, dw, dh) in enumerate(synth.resize_geometries(5, 2000)):
+        img = big[:sh, :sw] if k % 2 else np.full((sh, sw, 3), 255 * (k % 4 == 0), np.uint8)
+        want = cv2.resize(img, (dw, dh), interpolation=cv2.INTER_LINEAR)
+        assert (oracle.resize(img, dw, dh) == want).all(), (sw, sh, dw, dh)
+
+
 def test_resize_target_rules():
     # tests/test_ops.cpp:126-147
     assert oracle.resize_target(1920, 1080, 224, 224) == (224, 224)
