@@ -295,6 +295,12 @@ SCN_ENGINE_API int scn_db_save_job(scn_db* db, scn_job* j, const char* table, co
 SCN_ENGINE_API int scn_db_new_table(scn_db* db, const char* table, const char* column_name, int is_video,
                                     const char* type_name, int job_id); /* -> table id */
 SCN_ENGINE_API int scn_job_set_sink_table(scn_job* j, int sink, int table_id, int keep_rows);
+/* Store a sink's frames as H.264 (reference compress_video()): when the sink also has a table and runs on a GPU
+ * pipeline instance, each task's item becomes one intra-only H.264 stream at constant `qp` (0-51) with an IDR
+ * every `keyframe_distance` pictures from the task's first row (scn_h264_encode_u8), encoded on the instance's GPU
+ * before anything crosses to the host.  Frames must be 3-channel uint8 of one even size per task and no row may
+ * be null; anything else fails the run.  On CPU instances, and for sinks without a table, rows stay raw. */
+SCN_ENGINE_API int scn_job_set_sink_encoding(scn_job* j, int sink, int qp, int keyframe_distance);
 /* The same for many tables with ONE catalogue lock / rewrite per call (a job list with hundreds of output streams;
  * several ranks sharing the directory): n one-column tables -> out_ids[n]; commit of n (table, job) pairs; delete. */
 SCN_ENGINE_API int scn_db_new_tables(scn_db* db, int n, const char* const* tables, const char* const* column_names,

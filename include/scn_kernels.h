@@ -195,6 +195,27 @@ SCN_API int scn_jpeg_encode_u8(const uint8_t* const* host_src_ptrs, int n, int w
                                void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * H.264  (the save stage's video encoder: upstream, compress_video() outputs went through libavcodec).
+ *        Intra-only Baseline H.264 with CAVLC, every macroblock Intra16x16, constant QP, one slice per
+ *        picture, deblocking off.  oracle/h264_enc.py is the same encoder in integer numpy and documents every
+ *        decision (colour conversion, mode choice, quantisation); the output is byte for byte the oracle's.
+ * scn_h264_encode_u8: n dense RGB24 frames of one geometry, any base alignment -> n Annex-B access units.
+ *   positions[i] is frame i's position within its item (null: 0, 1, ..., n - 1): position p is an IDR
+ *   picture, with SPS and PPS in its access unit, when p % keyframe_distance == 0, and a non-IDR I picture
+ *   with frame_num (p % keyframe_distance) % 16 otherwise.  QP 0-51, keyframe_distance >= 1, positions >= 0,
+ *   else SCN_E_BADARG.  An odd width or height, a side over 4096 or more than 36,864 macroblocks (level
+ *   5.1's MaxFS): SCN_E_UNSUPPORTED.  Pointer list; batches over 64 frames are split into launches.
+ *   Scratch, the output callback, host_sizes and the two stream synchronisations are as in
+ *   scn_jpeg_encode_u8: access unit i is at the sum of the sizes before it in the buffer alloc_out returned.
+ * scn_h264_encode_bound: bytes no access unit of that geometry exceeds at any QP (0 for a geometry
+ *   scn_h264_encode_u8 refuses).
+ */
+SCN_API size_t scn_h264_encode_bound(int width, int height);
+SCN_API int scn_h264_encode_u8(const uint8_t* const* host_src_ptrs, int n, int width, int height, int qp,
+                               const int* host_positions, int keyframe_distance, scn_alloc_fn alloc_out,
+                               void* alloc_ctx, size_t* host_sizes, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * OpticalFlow  (replaces OpticalFlowKernelCPU::execute, tests/test_ops.cpp:79-98:
  *   cvtColor(COLOR_BGR2GRAY) on each RGB frame of the {0,1} stencil window, then
  *   cv::FarnebackOpticalFlow(numLevels, pyrScale, fastPyramids=false, winSize, numIters, polyN,

@@ -113,9 +113,10 @@ class OpColumn:
         self._op, self._col, self._is_frame = op, column, is_frame
         self._encode_options = encode_options
 
-    # How a frame column is stored when it reaches an Output (op.py:57-98).  There is no video encoder
-    # on the box (no NVENC library, no x264): every choice is recorded and the frames are stored
-    # uncompressed, i.e. `lossless()` is exact and `compress_video()` keeps more than it asked for.
+    # How a frame column is stored when it reaches an Output (op.py:57-98).  `compress_video()` on a client with
+    # GPUs and a database stores each task's frames as intra-only H.264 (scn_h264_encode_u8, on the pipeline
+    # instance's GPU); `lossless()`, `compress("default")` and unannotated columns are stored uncompressed, and so
+    # is everything on CPU-only clients and in clients without a database (their outputs stay in memory).
     def _stored_as(self, options):
         if not self._is_frame:
             raise ScannerException(f'Compression only supported for sequences of type "video". Sequence '
@@ -130,6 +131,10 @@ class OpColumn:
         return codecs[codec](**kwargs)
 
     def compress_video(self, quality=-1, bitrate=-1, keyframe_distance=-1):
+        """Store the frames as H.264 (3-channel uint8 frames of one even size per task, no null rows; anything
+        else fails the run).  quality: the constant QP, 0-51 (-1: 23, x264's default CRF); keyframe_distance:
+        pictures between IDRs (-1: 120, the reference encoder's gop_size).  bitrate is accepted and not honoured:
+        the encoder is constant-QP, without rate control."""
         return self._stored_as({"codec": "h264", "quality": quality, "bitrate": bitrate,
                                 "keyframe_distance": keyframe_distance})
 
@@ -138,6 +143,23 @@ class OpColumn:
 
     def compress_default(self):
         return self._stored_as({"codec": "default"})
+
+
+def _h264_encoding(col):
+    """compress_video() options of an output's column -> (QP, keyframe_distance); None when it is stored raw."""
+    opts = col._encode_options
+    if not opts or opts.get("codec") != "h264":
+        return None
+    q, kd = opts.get("quality", -1), opts.get("keyframe_distance", -1)
+    if q == -1:
+        q = 23
+    elif isinstance(q, bool) or not isinstance(q, int) or not 0 <= q <= 51:
+        raise ScannerException(f"compress_video(quality={q!r}): quality is the H.264 QP, 0-51 (or -1 for 23)")
+    if kd == -1:
+        kd = 120
+    elif isinstance(kd, bool) or not isinstance(kd, int) or kd < 1:
+        raise ScannerException(f"compress_video(keyframe_distance={kd!r}): at least 1 (or -1 for 120)")
+    return q, kd
 
 
 class SliceList(list):
@@ -498,10 +520,14 @@ class NamedVideoStream:
         return NamedStream.load_bytes(self, rows)
 
     def load(self, ty=None, fn=None, rows=None):
-        """Generator over frames (ndarrays).  Frames written by a job are stored uncompressed and
-        read back as they are; an ingested H.264 video is decoded for the asked rows (the reference
-        runs a Gather + ImageEncoder job for this, column.py:227-240; here the decode stage is
-        called directly, which needs a GPU)."""
+        """Generator over frames (ndarrays).  Frames a job stored uncompressed are read back as they are; an
+        ingested H.264 video, or a job output stored with compress_video(), is decoded for the asked rows (the
+        reference runs a Gather + ImageEncoder job for this, column.py:227-240; here the decode stage is called
+        directly, which needs a GPU).  A compressed job output of several items (one per task) reads as one
+        stream."""
+        if self._job is None and self._sid is None and self._stored() and \
+                self._sc._db.table_info(self._name)["keyframes"] > 0:
+            self._bind()
         if self._job is None and self._sid is not None and self._is_compressed():
             return self._decode(rows)
         return NamedStream.load(self, ty, fn, rows)
@@ -544,8 +570,8 @@ class NamedVideoStream:
 
     def save_mp4(self, output_name, fps=None):
         """Write the video as `<output_name>.mp4` (reference storage.py NamedVideoStream.save_mp4).
-        An ingested H.264 table is re-wrapped sample for sample.  Frames written by a job are stored
-        uncompressed here (there is no encoder on the box): they are converted to BT.601 4:2:0 and
+        An ingested H.264 table, or a job output stored with compress_video(), is re-wrapped sample for
+        sample without re-encoding.  Frames a job stored uncompressed are converted to BT.601 4:2:0 and
         written as intra-PCM H.264 -- every player opens it, the file is as large as the raw video."""
         path = output_name if output_name.endswith(".mp4") else output_name + ".mp4"
         db = self._sc._db
@@ -1007,6 +1033,7 @@ class Client:
             visit(o)
         # ---- output tables that already exist (reference CacheMode, client.py:1325-1370)
         out_nodes = [n for n in order if n.kind == "output"]
+        encodings = {id(n): _h264_encoding(n.inputs[0]) for n in out_nodes}
         skip = set()
         if self._db is not None and out_nodes:
             for j in range(len(out_nodes[0].streams)):
@@ -1087,6 +1114,8 @@ class Client:
                         tid = self._db.new_table(s.name(), src_col._col, src_col._is_frame, type_name, bulk_job_id)
                         reserved.append((tid, s.name(), jobs[job_of[j]]))
                         jobs[job_of[j]].set_sink_table(index[id(node)], tid, keep_rows=False)
+                        if encodings[id(node)] and self._gpus:
+                            jobs[job_of[j]].set_sink_encoding(index[id(node)], *encodings[id(node)])
             except E.EngineError as e:
                 for _, name, _ in reserved:
                     self._db.delete_table(name)

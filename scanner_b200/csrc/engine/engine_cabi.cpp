@@ -598,6 +598,13 @@ int scn_job_set_sink_table(scn_job* j, int sink, int table_id, int keep_rows) {
   return 0;
 }
 
+int scn_job_set_sink_encoding(scn_job* j, int sink, int qp, int keyframe_distance) {
+  if (!j || qp < 0 || qp > 51 || keyframe_distance < 1)
+    return fail("bad arguments: H.264 QP must be 0-51 and keyframe_distance at least 1");
+  j->j.sink_encoding[sink] = Job::SinkEncoding{qp, keyframe_distance};
+  return 0;
+}
+
 int scn_db_new_table(scn_db* db, const char* table, const char* column_name, int is_video, const char* type_name,
                      int job_id) {
   if (!db || !table || !column_name) return fail("bad arguments");

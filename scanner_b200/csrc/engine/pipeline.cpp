@@ -282,6 +282,98 @@ struct SourceCursor {
   }
 };
 
+// Post-evaluate of a sink stored as H.264 (Job::sink_encoding): the batch's frames, on the instance's GPU (host
+// frames are uploaded to it first), are encoded at positions pos0, pos0 + 1, ... of the task's item, and only the
+// access units cross to the host, appended to `to` as the rows.  Every element of `cb` is left to the caller.
+Result encode_h264_rows(const ColumnBatch& cb, i32 gpu, cudaStream_t stream, const Job::SinkEncoding& enc, i32 sink,
+                        TaskOutput& to) {
+  Result r = ok();
+  const size_t n = cb.elements.size();
+  if (n == 0) return r;
+  const i64 pos0 = (i64)to.sizes.size();
+  i32 w = pos0 ? to.shapes[1] : 0, h = pos0 ? to.shapes[0] : 0;
+  for (size_t i = 0; i < n; ++i) {
+    const Element& e = cb.elements[i];
+    std::string what;
+    const Frame* f = e.is_frame ? e.as_const_frame() : nullptr;
+    if (e.is_null()) {
+      what = "the row is null";
+    } else if (!f) {
+      what = "the row is not a frame";
+    } else if (f->shape[2] != 3 || f->type != FrameType::U8) {
+      what = "the frame is " + std::to_string(f->shape[1]) + "x" + std::to_string(f->shape[0]) + " with " +
+             std::to_string(f->shape[2]) + " channel(s) of type " + std::to_string((int)f->type);
+    } else if (f->shape[0] % 2 || f->shape[1] % 2) {
+      what = "the frame is " + std::to_string(f->shape[1]) + "x" + std::to_string(f->shape[0]) + ", an odd size";
+    } else if (w && (f->shape[1] != w || f->shape[0] != h)) {
+      what = "the frame is " + std::to_string(f->shape[1]) + "x" + std::to_string(f->shape[0]) +
+             ", earlier frames of its item are " + std::to_string(w) + "x" + std::to_string(h);
+    }
+    if (!what.empty()) {
+      RESULT_ERROR(&r, "sink %d, row %ld: %s.  compress_video() stores 3-channel uint8 frames of one even size and no "
+                       "null rows; store this column with .lossless()", sink, (long)cb.row_ids[i], what.c_str());
+      return r;
+    }
+    w = f->shape[1], h = f->shape[0];
+  }
+  if (!scn_h264_encode_bound(w, h)) {
+    RESULT_ERROR(&r, "sink %d: %dx%d frames are beyond H.264 level 5.1 (a side over 4096 or over 36,864 "
+                     "macroblocks); store this column with .lossless()", sink, w, h);
+    return r;
+  }
+  cudaSetDevice(gpu);
+  const DeviceHandle gdev(DeviceType::GPU, gpu);
+  const size_t fb = (size_t)w * h * 3;
+  std::vector<const u8*> src(n);
+  u8* staging = nullptr;
+  if (!cb.device.is_gpu()) {  // frames a CPU op left on the host
+    staging = new_buffer(gdev, n * fb);
+    for (size_t i = 0; i < n; ++i) {
+      src[i] = staging + i * fb;
+      cudaMemcpyAsync(staging + i * fb, cb.elements[i].as_const_frame()->data, fb, cudaMemcpyHostToDevice, stream);
+    }
+  } else {
+    for (size_t i = 0; i < n; ++i) src[i] = cb.elements[i].as_const_frame()->data;
+  }
+  std::vector<int> pos(n);
+  for (size_t i = 0; i < n; ++i) pos[i] = (int)(pos0 + (i64)i);
+  struct Out {
+    DeviceHandle dev;
+    u8* buf;
+  } out{gdev, nullptr};
+  auto alloc = [](void* ctx, size_t bytes) -> void* {
+    Out* o = static_cast<Out*>(ctx);
+    o->buf = new_buffer(o->dev, bytes ? bytes : 1);
+    return o->buf;
+  };
+  std::vector<size_t> sizes(n);
+  int rc = scn_h264_encode_u8(src.data(), (int)n, w, h, enc.qp, pos.data(), enc.keyframe_distance, alloc, &out,
+                              sizes.data(), stream);
+  size_t total = 0;
+  for (size_t z : sizes) total += z;
+  std::vector<u8> host(rc ? 0 : total);
+  if (!rc && total) rc = (int)cudaMemcpyAsync(host.data(), out.buf, total, cudaMemcpyDeviceToHost, stream);
+  if (!rc) rc = (int)cudaStreamSynchronize(stream);
+  if (out.buf) delete_buffer(gdev, out.buf);
+  if (staging) delete_buffer(gdev, staging);
+  if (rc) {
+    RESULT_ERROR(&r, "sink %d: H.264 encoding of rows %ld-%ld on GPU %d failed (status %d)", sink,
+                 (long)cb.row_ids.front(), (long)cb.row_ids.back(), gpu, rc);
+    return r;
+  }
+  const i32 shape[4] = {h, w, 3, (i32)(proto::FrameType)FrameType::U8};
+  size_t at = 0;
+  for (size_t i = 0; i < n; ++i) {
+    to.offsets.push_back(to.data.size());
+    to.sizes.push_back(sizes[i]);
+    to.shapes.insert(to.shapes.end(), shape, shape + 4);
+    to.data.insert(to.data.end(), host.begin() + at, host.begin() + at + sizes[i]);
+    at += sizes[i];
+  }
+  to.h264 = true;
+  return r;
+}
+
 }  // namespace
 
 void TaskOutput::release() {
@@ -607,6 +699,12 @@ void Engine::instance_main(Instance* inst) {
         // ---- post-evaluate + save: bring sink rows to the host and append them to the task
         for (auto& kv : sink_cols) {
           ColumnBatch& cb = kv.second;
+          const auto enc = job.sink_encoding.find(kv.first);
+          if (gpu >= 0 && enc != job.sink_encoding.end() && job.sink_tables.count(kv.first)) {
+            if (r.success()) r = encode_h264_rows(cb, gpu, stream, enc->second, kv.first, *outs[kv.first]);
+            delete_elements(cb.device, cb.elements);
+            continue;
+          }
           Elements host = cb.device.is_gpu() ? copy_or_ref_elements(cb.device, CPU_DEVICE, cb.elements) : cb.elements;
           TaskOutput& to = *outs[kv.first];
           for (Element& e : host) {
@@ -645,6 +743,7 @@ void Engine::instance_main(Instance* inst) {
           delete_elements(CPU_DEVICE, host);  // rows kept above were replaced by null elements
           if (cb.device.is_gpu()) delete_elements(cb.device, cb.elements);
         }
+        if (!r.success()) break;
       }
       // close decoder intervals left open by a task that did not need their tail
       for (SourceCursor& c : cursors) {
@@ -697,6 +796,7 @@ void Engine::instance_main(Instance* inst) {
             }
             ic.sizes = &to->sizes;
             ic.shapes = &to->shapes;
+            ic.h264 = to->h264;
             Result wr = rsp->db->write_index_item(table, task_id, row0, row1);
             if (wr.success()) wr = rsp->db->write_item(table, 1, task_id, ic, video);
             if (!wr.success()) {

@@ -76,6 +76,7 @@ struct TaskOutput {
   std::vector<const u8*> ext;    // per row: non-null = the row lives in a held host block
   Elements held;                 // host elements that keep those blocks alive
   bool dropped = false;          // payload written to a table and released (sizes/shapes remain)
+  bool h264 = false;             // rows are the H.264 access units of the task's frames (one item per task)
 
   TaskOutput() = default;
   TaskOutput(const TaskOutput&) = delete;
@@ -92,6 +93,7 @@ struct TaskOutput {
       ext = std::move(o.ext);
       held = std::move(o.held);
       dropped = o.dropped;
+      h264 = o.h264;
       o.held.clear();
     }
     return *this;
@@ -123,6 +125,14 @@ struct Job {
   // keep_rows == false the rows of such sinks are dropped from memory once their item is written.
   std::map<i32, i32> sink_tables;
   bool keep_rows = true;
+  // sink op -> H.264 encoding of its frames (scn_job_set_sink_encoding).  Applies to a sink in sink_tables on a
+  // GPU pipeline instance: each task's item is then one intra-only H.264 stream (scn_h264_encode_u8) instead of
+  // raw frames.
+  struct SinkEncoding {
+    i32 qp = 23;
+    i32 keyframe_distance = 120;
+  };
+  std::map<i32, SinkEncoding> sink_encoding;
   // One clip split into contiguous output-row intervals across ranks (configs[3]): this job computes
   // rows [shard_bounds[shard_index], shard_bounds[shard_index + 1]) only; shard q is computed by rank
   // shard_ranks[q].  Source rows a stencil reaches into a neighbouring interval are not decoded here:

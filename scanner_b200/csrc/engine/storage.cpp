@@ -282,6 +282,26 @@ Result Database::write_index_item(i32 table_id, i32 item_id, i64 row0, i64 row1)
   return write_item(table_id, 0, item_id, c, false);
 }
 
+// The H.264 part of a VideoDescriptor from the index of its `bytes`-byte stream (reference ingest.cpp:211-224,
+// 347-366): ingested videos and the items of compressed job outputs are described alike.
+static void describe_h264(const H264Index& idx, size_t bytes, tables::VideoDescriptor& vd) {
+  vd.set_frames(idx.frames());
+  vd.set_width(idx.width);
+  vd.set_height(idx.height);
+  vd.set_channels(3);
+  vd.set_frame_type((int)proto::U8);
+  vd.set_codec_type(0);
+  vd.set_chroma_format(1);
+  vd.set_num_encoded_videos(1);
+  vd.add_frames_per_video(idx.frames());
+  vd.add_keyframes_per_video((i64)idx.keyframe_indices.size());
+  vd.add_size_per_video((i64)bytes);
+  for (u64 v : idx.sample_offsets) vd.add_sample_offsets(v);
+  for (u64 v : idx.sample_sizes) vd.add_sample_sizes(v);
+  for (i64 v : idx.keyframe_indices) vd.add_keyframe_indices((u64)v);
+  vd.mutable_metadata_packets()->assign((const char*)idx.metadata_packets.data(), idx.metadata_packets.size());
+}
+
 Result Database::write_item(i32 table_id, i32 column_id, i32 item_id, const ItemColumn& col, bool is_video) {
   Result r = ok();
   const std::string base = item_base(table_id, column_id, item_id);
@@ -304,12 +324,29 @@ Result Database::write_item(i32 table_id, i32 column_id, i32 item_id, const Item
       RESULT_ERROR(&r, "cannot write %s_metadata.bin: %s", base.c_str(), strerror(errno));
     return r;
   }
-  // frame column stored uncompressed (reference column_sink.cpp:159-176): codec RAW, one "sample"
-  // per frame so rows stay addressable; null rows have size 0
   tables::VideoDescriptor vd;
   vd.set_table_id(table_id);
   vd.set_column_id(column_id);
   vd.set_item_id(item_id);
+  if (col.h264) {
+    // the rows are the access units of one stream (scn_job_set_sink_encoding): indexed like an ingested video
+    H264Index idx;
+    r = index_bytestream(col.data, col.bytes, idx);
+    if (!r.success()) return r;
+    if ((size_t)idx.frames() != sizes.size()) {
+      RESULT_ERROR(&r, "item %d of table %d: %ld pictures in the H.264 stream of %zu rows", item_id, table_id,
+                   (long)idx.frames(), sizes.size());
+      return r;
+    }
+    describe_h264(idx, col.bytes, vd);
+    vd.set_data_path(base + ".bin");
+    const std::string s = vd.SerializeAsString();
+    if (!write_file_atomic(base + "_video_metadata.bin", s.data(), s.size()))
+      RESULT_ERROR(&r, "cannot write %s_video_metadata.bin: %s", base.c_str(), strerror(errno));
+    return r;
+  }
+  // frame column stored uncompressed (reference column_sink.cpp:159-176): codec RAW, one "sample"
+  // per frame so rows stay addressable; null rows have size 0
   vd.set_frames((i64)sizes.size());
   vd.set_codec_type(2);
   vd.set_chroma_format(1);
@@ -452,27 +489,13 @@ Result Database::ingest_h264(const std::string& table, const u8* annexb, size_t 
       return r;
     }
   }
-  tables::VideoDescriptor vd;  // reference ingest.cpp:211-224, 347-366
+  tables::VideoDescriptor vd;
   vd.set_table_id(id);
   vd.set_column_id(1);
   vd.set_item_id(0);
-  vd.set_frames(idx.frames());
-  vd.set_width(idx.width);
-  vd.set_height(idx.height);
-  vd.set_channels(3);
-  vd.set_frame_type((int)proto::U8);
-  vd.set_codec_type(0);
-  vd.set_chroma_format(1);
+  describe_h264(idx, size, vd);
   vd.set_time_base_num(tb_num);
   vd.set_time_base_denom(tb_den);
-  vd.set_num_encoded_videos(1);
-  vd.add_frames_per_video(idx.frames());
-  vd.add_keyframes_per_video((i64)idx.keyframe_indices.size());
-  vd.add_size_per_video((i64)size);
-  for (u64 v : idx.sample_offsets) vd.add_sample_offsets(v);
-  for (u64 v : idx.sample_sizes) vd.add_sample_sizes(v);
-  for (i64 v : idx.keyframe_indices) vd.add_keyframe_indices((u64)v);
-  vd.mutable_metadata_packets()->assign((const char*)idx.metadata_packets.data(), idx.metadata_packets.size());
   vd.set_data_path(inplace_path.empty() ? base + ".bin" : inplace_path);
   vd.set_inplace(!inplace_path.empty());
   const std::string s = vd.SerializeAsString();
@@ -500,7 +523,7 @@ Result Database::read_table(const std::string& table, tables::TableDescriptor& o
 }
 
 Result Database::read_video(const std::string& table, tables::VideoDescriptor& out, std::string& data_file,
-                            const std::string& column) const {
+                            const std::string& column, std::vector<std::string>* item_files) const {
   tables::TableDescriptor td;
   Result r = read_table(table, td);
   if (!r.success()) return r;
@@ -514,22 +537,71 @@ Result Database::read_video(const std::string& table, tables::VideoDescriptor& o
     RESULT_ERROR(&r, "table %s has no video column %s", table.c_str(), column.c_str());
     return r;
   }
-  const std::string base = item_base(td.id(), col, 0);
-  std::string bytes;
-  if (!read_file(base + "_video_metadata.bin", bytes) || !out.ParseFromString(bytes)) {
-    RESULT_ERROR(&r, "cannot read %s_video_metadata.bin", base.c_str());
-    return r;
+  auto read_item = [&](i32 item, tables::VideoDescriptor& vd) {
+    const std::string base = item_base(td.id(), col, item);
+    std::string bytes;
+    if (!read_file(base + "_video_metadata.bin", bytes) || !vd.ParseFromString(bytes))
+      RESULT_ERROR(&r, "cannot read %s_video_metadata.bin", base.c_str());
+    // the stored data_path is absolute for the writer's mount point; the file next to the
+    // descriptor is authoritative (a database directory can be moved)
+    return base + ".bin";
+  };
+  data_file = read_item(0, out);
+  if (item_files) item_files->assign(1, data_file);
+  if (!r.success() || out.codec_type() != 0 || td.end_rows_size() <= 1) return r;
+  // A job writes one item per task, so a compressed output column has several: they read as one stream, samples
+  // back to back, keyframe indices offset by each item's first row.
+  i64 bytes = out.size_per_video_size() ? out.size_per_video(0) : 0;
+  for (i32 item = 1; item < td.end_rows_size(); ++item) {
+    tables::VideoDescriptor vd;
+    const std::string file = read_item(item, vd);
+    if (!r.success()) return r;
+    const i64 first = td.end_rows(item - 1);
+    if (vd.codec_type() != 0 || vd.width() != out.width() || vd.height() != out.height() || first != out.frames() ||
+        vd.size_per_video_size() != 1) {
+      RESULT_ERROR(&r, "item %d of video column %d of table %s (%s, %dx%d, from row %ld) does not continue item 0's "
+                       "H.264 stream (%dx%d, %ld rows before it): the items of a compressed column must share one "
+                       "geometry to be read as one stream", item, col, table.c_str(),
+                   vd.codec_type() == 0 ? "H.264" : "not H.264", vd.width(), vd.height(), (long)first, out.width(),
+                   out.height(), (long)out.frames());
+      return r;
+    }
+    for (u64 o : vd.sample_offsets()) out.add_sample_offsets(o + (u64)bytes);
+    for (u64 z : vd.sample_sizes()) out.add_sample_sizes(z);
+    for (u64 k : vd.keyframe_indices()) out.add_keyframe_indices(k + (u64)first);
+    out.set_frames(out.frames() + vd.frames());
+    bytes += vd.size_per_video(0);
+    if (item_files) item_files->push_back(file);
   }
-  // the stored data_path is absolute for the writer's mount point; the file next to the
-  // descriptor is authoritative (a database directory can be moved)
-  data_file = base + ".bin";
+  out.clear_frames_per_video();
+  out.add_frames_per_video(out.frames());
+  out.clear_keyframes_per_video();
+  out.add_keyframes_per_video(out.keyframe_indices_size());
+  out.clear_size_per_video();
+  out.add_size_per_video(bytes);
   return r;
 }
 
 Result Database::load_video(const std::string& table, tables::VideoDescriptor& vd, std::vector<u8>& annexb) const {
   std::string file;
-  Result r = read_video(table, vd, file);
+  std::vector<std::string> items;
+  Result r = read_video(table, vd, file, "", &items);
   if (!r.success()) return r;
+  if (items.size() > 1) {  // a compressed job output: its items back to back
+    annexb.clear();
+    for (const std::string& f : items) {
+      std::string part;
+      if (!read_file(f, part)) {
+        RESULT_ERROR(&r, "cannot read %s (video data of table %s): %s", f.c_str(), table.c_str(), strerror(errno));
+        return r;
+      }
+      annexb.insert(annexb.end(), part.begin(), part.end());
+    }
+    if ((i64)annexb.size() != vd.size_per_video(0))
+      RESULT_ERROR(&r, "table %s: its items hold %zu stream bytes, their descriptors %ld", table.c_str(),
+                   annexb.size(), (long)vd.size_per_video(0));
+    return r;
+  }
   if (vd.inplace()) file = vd.data_path();
   std::string bytes;
   if (!read_file(file, bytes)) {

@@ -38,6 +38,7 @@ struct ItemColumn {
   size_t bytes = 0;
   const std::vector<u64>* sizes = nullptr;   // per row
   const std::vector<i32>* shapes = nullptr;  // 4 per row (h, w, c, frame type), frame columns only
+  bool h264 = false;                         // the rows are the access units of one H.264 stream
 };
 
 class Database {
@@ -66,9 +67,11 @@ class Database {
 
   // ---- read side
   Result read_table(const std::string& table, tables::TableDescriptor& out) const;
-  // descriptor of video column `column` (default: the first Video column) and its data file
+  // descriptor of video column `column` (default: the first Video column) and its data file.  A compressed column
+  // of several items (a job's output, one item per task) is described as one stream over all of them; item_files
+  // then lists their data files in order.
   Result read_video(const std::string& table, tables::VideoDescriptor& out, std::string& data_file,
-                    const std::string& column = "") const;
+                    const std::string& column = "", std::vector<std::string>* item_files = nullptr) const;
   // rows of a column -> concatenated bytes + per-row sizes (+ shapes for frame columns)
   Result read_rows(const std::string& table, const std::string& column, const std::vector<i64>& rows,
                    std::vector<u8>& data, std::vector<u64>& sizes, std::vector<i32>& shapes) const;

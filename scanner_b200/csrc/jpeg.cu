@@ -24,8 +24,6 @@
 #include <cuda_runtime.h>
 
 #include <cstring>
-#include <map>
-#include <mutex>
 #include <vector>
 
 #include "scn_common.cuh"
@@ -308,32 +306,6 @@ __device__ __forceinline__ uint64_t fdct_quant(const uint32_t* qmag, const uint1
 
 __device__ __forceinline__ int bit_length(int v) { return 32 - __clz(abs(v)); }
 
-// Appends bits MSB first to a frame's bit stream of big-endian 32-bit words.  The first and the last word a
-// writer touches may be shared with the neighbouring MCUs and are ORed in; the words between are its own.
-struct BitWriter {
-  uint32_t* words;
-  uint64_t word;  // index of the word being filled
-  uint64_t acc;   // the low n bits are pending
-  int n;
-  bool first;
-  __device__ BitWriter(uint32_t* w, uint64_t bit) : words(w), word(bit >> 5), acc(0), n((int)(bit & 31)), first(true) {}
-  __device__ __forceinline__ void put(uint32_t bits, int len) {  // len <= 27
-    acc = (acc << len) | bits;
-    n += len;
-    if (n >= 32) {
-      n -= 32;
-      const uint32_t v = __byte_perm((uint32_t)(acc >> n), 0, 0x0123);
-      if (first) atomicOr(words + word, v);
-      else words[word] = v;
-      first = false;
-      ++word;
-    }
-  }
-  __device__ __forceinline__ void finish() {
-    if (n) atomicOr(words + word, __byte_perm((uint32_t)(acc << (32 - n)), 0, 0x0123));
-  }
-};
-
 // bits of the AC symbols of one block (zz in shared memory, nz its nonzero AC mask); with W, also writes them
 template <bool Emit>
 __device__ __forceinline__ uint32_t code_ac(const int16_t* zz, uint64_t nz, const uint32_t* ac, BitWriter* bw) {
@@ -455,36 +427,6 @@ jpeg_mcu_kernel(PtrBatch srcs, int i0, Geom g, const __grid_constant__ Tables ta
   }
 }
 
-// block-wide exclusive scan of one value per thread (blockDim.x a multiple of 32, at most 1024); returns the
-// exclusive prefix, *total the block's sum.  Every thread of the block calls it.
-template <class T>
-__device__ __forceinline__ T block_exclusive_scan(T v, T* total) {
-  __shared__ T warp_sums[32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  T x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const T y = __shfl_up_sync(0xFFFFFFFFu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp_sums[wid] = x;
-  __syncthreads();
-  if (wid == 0) {
-    T s = lane < nw ? warp_sums[lane] : 0;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const T y = __shfl_up_sync(0xFFFFFFFFu, s, o);
-      if (lane >= o) s += y;
-    }
-    warp_sums[lane] = s;  // inclusive
-  }
-  __syncthreads();
-  const T before = wid ? warp_sums[wid - 1] : 0;
-  *total = warp_sums[nw - 1];
-  __syncthreads();  // warp_sums is reused by the next call
-  return before + x - v;
-}
-
 // One CTA per frame: MCU bit counts (AC bits + DC difference bits) -> bit offsets, and the frame's total.
 __global__ void __launch_bounds__(1024)
 jpeg_scan_kernel(int i0, uint32_t nm, int bpm, Tables tables, const int16_t* dcs_all, const uint32_t* acbits_all,
@@ -585,42 +527,6 @@ jpeg_stuff_kernel(const __grid_constant__ StreamSlots s, const __grid_constant__
     o[1] = 0xD9;
   }
 }
-
-// ---- device scratch: a stream-ordered pool per device, kept by the library ----
-cudaMemPool_t scratch_pool() {
-  static std::mutex mu;
-  static std::map<int, cudaMemPool_t> pools;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
-  std::lock_guard<std::mutex> lock(mu);
-  auto it = pools.find(dev);
-  if (it != pools.end()) return it->second;
-  cudaMemPoolProps props = {};
-  props.allocType = cudaMemAllocationTypePinned;
-  props.location.type = cudaMemLocationTypeDevice;
-  props.location.id = dev;
-  cudaMemPool_t pool = nullptr;
-  if (cudaMemPoolCreate(&pool, &props) != cudaSuccess) return nullptr;
-  uint64_t keep = ~0ull;  // keep freed scratch for the next call instead of returning it at every synchronisation
-  cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-  pools[dev] = pool;
-  return pool;
-}
-
-struct Scratch {
-  cudaStream_t st;
-  std::vector<void*> held;
-  ~Scratch() {
-    for (void* p : held) cudaFreeAsync(p, st);
-  }
-  template <class T>
-  T* get(size_t count, cudaMemPool_t pool) {
-    void* p = nullptr;
-    if (cudaMallocFromPoolAsync(&p, count * sizeof(T) + 16, pool, st) != cudaSuccess) return nullptr;
-    held.push_back(p);
-    return static_cast<T*>(p);
-  }
-};
 
 size_t worst_bits_per_block() { return 11 + 11 + 63 * (16 + 10); }  // DC code + value, 63 AC codes + values
 

@@ -84,6 +84,7 @@ SIGNATURES = {
     "scn_db_save_job": (_I, [_VP, _VP, _CP, _IP, _c.POINTER(_CP), _c.POINTER(_CP), _I, _I]),
     "scn_db_new_table": (_I, [_VP, _CP, _CP, _I, _CP, _I]),
     "scn_job_set_sink_table": (_I, [_VP, _I, _I, _I]),
+    "scn_job_set_sink_encoding": (_I, [_VP, _I, _I, _I]),
     "scn_db_new_tables": (_I, [_VP, _I, _c.POINTER(_CP), _c.POINTER(_CP), _IP, _c.POINTER(_CP), _IP, _IP]),
     "scn_db_commit_job_tables": (_I, [_VP, _I, _IP, _c.POINTER(_VP)]),
     "scn_db_delete_tables": (_I, [_VP, _I, _c.POINTER(_CP)]),
@@ -612,6 +613,10 @@ class Job:
 
     def set_sink_table(self, sink, table_id, keep_rows=False):
         check(lib().scn_job_set_sink_table(self._h, sink, table_id, 1 if keep_rows else 0), "set_sink_table")
+
+    def set_sink_encoding(self, sink, qp=23, keyframe_distance=120):
+        """Store the sink's frames as intra-only H.264 at constant QP (scn_job_set_sink_encoding)."""
+        check(lib().scn_job_set_sink_encoding(self._h, sink, int(qp), int(keyframe_distance)), "set_sink_encoding")
 
     def set_stream_args(self, op, args):
         buf = ctypes.create_string_buffer(args, len(args)) if args else None

@@ -275,6 +275,70 @@ def jpeg_encode(frames, quality=95):
     return outs
 
 
+def h264_encode_bound(width, height):
+    """Bytes no access unit of that geometry exceeds at any QP (scn_h264_encode_bound); 0 if it is refused."""
+    return cabi.lib().scn_h264_encode_bound(width, height)
+
+
+def h264_encode(frames, qp=23, keyframe_distance=120, positions=None):
+    """Intra-only Baseline H.264 (CAVLC, constant QP) of RGB frames: one Annex-B access unit per frame, the bytes
+    oracle/h264_enc.py writes.  Frame i is at position positions[i] of its item (default 0, 1, ...): an IDR picture
+    with SPS and PPS when the position is a multiple of keyframe_distance, a non-IDR I picture otherwise, so the
+    concatenated access units of one item are a stream any H.264 decoder plays.
+
+    frames: (N,H,W,3) uint8 CUDA tensor or a list of (H,W,3) tensors of one shape; a frame need not be aligned.
+    Width and height even, each side at most 4096 and at most 36,864 macroblocks; QP 0-51.  -> list of N bytes
+    objects.  Synchronises the current stream."""
+    if isinstance(frames, torch.Tensor):
+        _need_cuda(frames)
+        if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+            raise cabi.ScnError(f"h264_encode takes (N,H,W,3) uint8 frames, got {tuple(frames.shape)} {frames.dtype}")
+        frames = frames.contiguous()
+        n, h, w, _ = frames.shape
+        ptrs = [frames.data_ptr() + i * h * w * 3 for i in range(n)]
+        device = frames.device
+    else:
+        lst = [t.contiguous() for t in frames]
+        _need_cuda(*lst)
+        if any(t.dtype != torch.uint8 or t.dim() != 3 or t.shape != lst[0].shape or t.shape[2] != 3 for t in lst):
+            raise cabi.ScnError("h264_encode takes (H,W,3) uint8 frames of one shape")
+        n = len(lst)
+        h, w = (lst[0].shape[0], lst[0].shape[1]) if n else (0, 0)
+        ptrs = [t.data_ptr() for t in lst]
+        device = lst[0].device if n else None
+    if n == 0:
+        return []
+    if not 0 <= int(qp) <= 51:
+        raise cabi.ScnError(f"h264_encode: QP {qp} is outside 0-51")
+    if int(keyframe_distance) < 1:
+        raise cabi.ScnError(f"h264_encode: keyframe_distance {keyframe_distance} is below 1")
+    if w % 2 or h % 2:
+        raise cabi.ScnError(f"h264_encode: {w}x{h} frames have an odd side (4:2:0 needs even sizes)")
+    if h264_encode_bound(w, h) == 0:
+        raise cabi.ScnError(f"h264_encode: {w}x{h} is beyond level 5.1 (a side over 4096 or over 36,864 macroblocks)")
+    if positions is not None and len(positions) != n:
+        raise cabi.ScnError(f"h264_encode: {len(positions)} positions for {n} frames")
+    keep = []
+
+    def alloc(_ctx, nbytes):
+        keep.append(torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device))
+        return keep[-1].data_ptr()
+
+    cb = cabi.ALLOC_FN(alloc)
+    sizes = (ctypes.c_size_t * n)()
+    pos = None if positions is None else (ctypes.c_int * n)(*[int(p) for p in positions])
+    sp, k1 = cabi.ptr_array(ptrs)
+    rc = cabi.lib().scn_h264_encode_u8(sp, n, w, h, int(qp), pos, int(keyframe_distance), cb, None, sizes,
+                                       _stream())
+    cabi.check(rc, "scn_h264_encode_u8")
+    data = keep[0].cpu().numpy().tobytes()  # on the current stream, after the access units are written
+    out, at = [], 0
+    for s in sizes:
+        out.append(data[at:at + s])
+        at += s
+    return out
+
+
 def optical_flow_sequence(frames, workspace=None, pairs_per_call=None):
     """Flow of every consecutive pair of a clip: (N,H,W,3) uint8 -> (N-1,H,W,2) float32.  Every frame is expanded
     once (scn_farneback_u8c3_chain); pairs_per_call splits the clip over several calls on one workspace, the way
