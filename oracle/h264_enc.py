@@ -600,6 +600,37 @@ def content(kind, h, w, seed):
 SWEEP_CONTENT = ("noise", "gradient", "flat", "saturated", "checkerboard", "stripes")
 
 
+def natural(h, w, seed):
+    """smooth fields plus mild noise: content where the quantiser, not the source, decides the quality"""
+    rng = np.random.default_rng(seed)
+    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
+    planes = []
+    for c in range(3):
+        f = sum(np.sin(rng.uniform(0.01, 0.08) * xx + rng.uniform(0.01, 0.08) * yy + rng.uniform(0, 6)) for _ in range(4))
+        planes.append(128 + 28 * f + rng.normal(0, 4, (h, w)))
+    return np.clip(np.stack(planes, -1), 0, 255).astype(np.uint8)
+
+
+# ---- the float reference the integer colour stage approximates -------------------------------------------------
+def bt601_float(rgb):
+    """BT.601 studio range in float64, from Kr = 0.299 and Kb = 0.114 (not from the integer coefficients above):
+    (..., 3) RGB -> Y, Cb, Cr.  Pass 2x2 block means to get 4:2:0 chroma."""
+    kr, kb = 0.299, 0.114
+    x = np.asarray(rgb, np.float64)
+    r, g, b = x[..., 0], x[..., 1], x[..., 2]
+    y = kr * r + (1 - kr - kb) * g + kb * b
+    return (16 + 219 / 255 * y, 128 + 224 / 255 * (b - y) / (2 - 2 * kb), 128 + 224 / 255 * (r - y) / (2 - 2 * kr))
+
+
+def bt601_planes(frame):
+    """(H, W, 3) uint8 frame, H and W even -> float64 Y (H, W) and Cb, Cr (H / 2, W / 2), each chroma sample from
+    the mean of its 2x2 block: what an exact encoder's planes would hold before rounding"""
+    h, w, _ = frame.shape
+    y = bt601_float(frame)[0]
+    _, cb, cr = bt601_float(frame.astype(np.float64).reshape(h // 2, 2, w // 2, 2, 3).mean((1, 3)))
+    return y, cb, cr
+
+
 def sweep():
     """(name, frames (3, H, W, 3), qp) over SWEEP_SIZES x SWEEP_CONTENT x SWEEP_QPS; encode them as one item with
     keyframe_distance 2 (IDR, non-IDR I, IDR)."""

@@ -62,19 +62,8 @@ def test_ffmpeg_decodes_1080p_noise_to_the_oracles_reconstruction(tmp_path):
     assert (y == recs[0][0]).all()
 
 
-def _natural(h, w, seed):
-    """smooth fields plus mild noise: content where the quantiser, not the source, decides the quality"""
-    rng = np.random.default_rng(seed)
-    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
-    planes = []
-    for c in range(3):
-        f = sum(np.sin(rng.uniform(0.01, 0.08) * xx + rng.uniform(0.01, 0.08) * yy + rng.uniform(0, 6)) for _ in range(4))
-        planes.append(128 + 28 * f + rng.normal(0, 4, (h, w)))
-    return np.clip(np.stack(planes, -1), 0, 255).astype(np.uint8)
-
-
 def test_size_and_psnr_fall_as_qp_rises(tmp_path):
-    frame = _natural(144, 176, 3)
+    frame = H.natural(144, 176, 3)
     src = H.rgb_to_planes(frame)[0][:144, :176]
     sizes, psnrs = [], []
     for qp in (0, 12, 23, 35, 51):
