@@ -266,6 +266,30 @@ SCN_API int scn_farneback_u8c3_chain(const uint8_t* const* host_prev_ptrs, const
  * overwritten. */
 SCN_API int scn_frame_digest(const uint8_t* const* host_ptrs, int n, size_t bytes, uint64_t* out, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * TV-L1 dense optical flow (no counterpart in the reference; DESIGN.md "TV-L1" is the specification): the
+ * Zach-Pock-Bischof duality scheme of Sanchez Perez et al. (IPOL 2013) with OpenCV DualTVL1OpticalFlow's
+ * parameter names and defaults (tau 0.25, lambda 0.15, theta 0.3, nscales 5, warps 5, epsilon 0.01,
+ * iterations 300, scale_step 0.8, median_filtering 5), gamma = 0.
+ * n pairs of dense u8 gray frames (prev_i, next_i), all width x height -> n float32 [height][width][2] flows
+ * (dx, dy) with prev(x, y) ~ next(x + dx, y + dy).  Pointer lists; any n (batches over 64 pairs run in 64-pair
+ * chunks).  Every (level, warp) step is one launch per kernel for all pairs of a chunk; the iterations of a
+ * step run inside one cooperative kernel that decides each pair's stop on the device.  Nothing synchronises
+ * with the host unless host_iterations is non-NULL: then it receives int [n][nscales][warps], level 0
+ * (finest) first, the iterations each (pair, level, warp) ran (0 for levels the pyramid stops before), and
+ * the call waits for the stream.  A pair's flow does not depend on the other pairs of the call (bit for bit).
+ * Refused with SCN_E_BADARG before any launch: a non-finite float, tau, lambda or theta <= 0,
+ * nscales outside 1-10, warps outside 1-20, iterations outside 1-10000, scale_step outside (0, 1),
+ * median_filtering other than 1, 3, 5, a side under 2, n < 0, a null pointer list or workspace, or
+ * workspace_bytes < scn_tvl1_workspace_bytes(width, height, n).  epsilon <= 0 disables the early stop.
+ */
+SCN_API size_t scn_tvl1_workspace_bytes(int width, int height, int n);
+SCN_API int scn_tvl1_u8(const uint8_t* const* host_prev_ptrs, const uint8_t* const* host_next_ptrs, int n,
+                        int width, int height, float* const* host_flow_ptrs, float tau, float lambda, float theta,
+                        int nscales, int warps, float epsilon, int iterations, float scale_step,
+                        int median_filtering, int* host_iterations, void* workspace, size_t workspace_bytes,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif

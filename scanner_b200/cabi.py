@@ -55,6 +55,10 @@ SIGNATURES = {
     "scn_h264_encode_bound": (_c.c_size_t, [_c.c_int, _c.c_int]),
     "scn_h264_encode_u8": (_c.c_int, [_PP, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.POINTER(_c.c_int), _c.c_int,
                                       ALLOC_FN, _VP, _c.POINTER(_c.c_size_t), _VP]),
+    "scn_tvl1_workspace_bytes": (_c.c_size_t, [_c.c_int, _c.c_int, _c.c_int]),
+    "scn_tvl1_u8": (_c.c_int, [_PP, _PP, _c.c_int, _c.c_int, _c.c_int, _PP, _c.c_float, _c.c_float, _c.c_float,
+                               _c.c_int, _c.c_int, _c.c_float, _c.c_int, _c.c_float, _c.c_int, _c.POINTER(_c.c_int),
+                               _VP, _c.c_size_t, _VP]),
 }
 
 _lib = None

@@ -901,6 +901,7 @@ class Client:
             self._op_protos["Resize"] = {"stream": std["ResizeArgs"]}
             self._op_protos["ConvertColor"] = {"stream": std["ConvertColorArgs"]}
             self._op_protos["ImageEncoder"] = {"init": std["ImageEncoderArgs"]}
+            self._op_protos["OpticalFlowTVL1"] = {"init": std["OpticalFlowTVL1Args"]}
 
     # ---- table catalogue (reference client.py: ingest_videos :1009-1078, has_table, delete_table)
     def _need_db(self):

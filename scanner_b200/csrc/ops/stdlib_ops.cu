@@ -415,6 +415,169 @@ REGISTER_KERNEL(OpticalFlow, OpticalFlowKernelGPU)
     .input_layout("frame", FrameLayout::NV12);
 
 // ---------------------------------------------------------------------------------------------
+// OpticalFlowTVL1: stencil {0,1}, TV-L1 dense flow (scn_tvl1_u8, DESIGN.md "TV-L1"), output Frame(H, W, 2, F32).
+// Not a reference op.  A batch of up to 8 windows is one scn_tvl1_u8 call; each distinct input frame of the batch
+// is converted to gray once (COLOR_RGB2GRAY from RGB24 or NV12 elements; 1-channel u8 frames are used as they are).
+class OpticalFlowTVL1KernelGPU : public StenciledBatchedKernel {
+ public:
+  OpticalFlowTVL1KernelGPU(const KernelConfig& config) : StenciledBatchedKernel(config), device_(config.devices[0]) {
+    OpticalFlowTVL1Args a;
+    if (!a.ParseFromArray(config.args.data(), (int)config.args.size())) {
+      args_problem_ = "could not parse OpticalFlowTVL1Args";
+      return;
+    }
+    // 0 (absent) means the default; a negative epsilon disables the early stop
+    tau_ = a.tau() != 0.f ? a.tau() : 0.25f;
+    lambda_ = a.lambda_() != 0.f ? a.lambda_() : 0.15f;
+    theta_ = a.theta() != 0.f ? a.theta() : 0.3f;
+    nscales_ = a.nscales() != 0 ? a.nscales() : 5;
+    warps_ = a.warps() != 0 ? a.warps() : 5;
+    epsilon_ = a.epsilon() != 0.f ? (a.epsilon() < 0.f ? -1.f : a.epsilon()) : 0.01f;
+    iterations_ = a.iterations() != 0 ? a.iterations() : 300;
+    scale_step_ = a.scale_step() != 0.f ? a.scale_step() : 0.8f;
+    median_ = a.median_filtering() != 0 ? a.median_filtering() : 5;
+    if (call(nullptr, nullptr, 0, 16, 16, nullptr) != 0)
+      args_problem_ = "invalid arguments (tau " + std::to_string(tau_) + ", lambda " + std::to_string(lambda_) +
+                      ", theta " + std::to_string(theta_) + ", nscales " + std::to_string(nscales_) + ", warps " +
+                      std::to_string(warps_) + ", epsilon " + std::to_string(epsilon_) + ", iterations " +
+                      std::to_string(iterations_) + ", scale_step " + std::to_string(scale_step_) +
+                      ", median_filtering " + std::to_string(median_) + ")";
+  }
+  ~OpticalFlowTVL1KernelGPU() {
+    if (workspace_) delete_buffer(device_, workspace_);
+    if (gray_) delete_buffer(device_, gray_);
+  }
+
+  void execute(const StenciledBatchedElements& input_columns, BatchedElements& output_columns) override {
+    const std::vector<Elements>& windows = input_columns[0];
+    const size_t nb = windows.size();
+    if (nb == 0) return;
+    CU_CHECK(cudaSetDevice(device_.id));
+    // runs of windows of one geometry
+    auto first = [&](size_t q) { return windows[q][0].is_null() ? nullptr : windows[q][0].as_const_frame(); };
+    size_t i = 0;
+    while (i < nb) {
+      const Frame* f0 = first(i);
+      size_t j = i + 1;
+      while (f0 && j < nb && first(j) && first(j)->as_frame_info() == f0->as_frame_info()) ++j;
+      run(windows, i, j, output_columns[0]);
+      i = j;
+    }
+  }
+
+ private:
+  int call(const u8* const* prev, const u8* const* next, int n, int w, int h, float* const* flow) {
+    return scn_tvl1_u8(prev, next, n, w, h, flow, tau_, lambda_, theta_, nscales_, warps_, epsilon_, iterations_,
+                       scale_step_, median_, nullptr, workspace_, workspace_bytes_, device_stream(device_));
+  }
+
+  static std::string frame_problem(const Frame* f) {
+    if ((proto::FrameType)f->type != proto::U8)
+      return "expects uint8 frames, got type " + std::to_string((int)(proto::FrameType)f->type);
+    if (is_nv12(f)) {
+      if (f->channels() != 1 || f->height() % 3 != 0 || (f->width() & 1))
+        return "malformed NV12 frame element " + std::to_string(f->height()) + "x" + std::to_string(f->width());
+    } else if (f->channels() != 1 && f->channels() != 3) {
+      return "expects gray (HxWx1), RGB24 (HxWx3) or NV12 frames, got " + std::to_string(f->height()) + "x" +
+             std::to_string(f->width()) + "x" + std::to_string(f->channels());
+    }
+    if (pic_width(f) < 2 || pic_height(f) < 2)
+      return "frames must be at least 2x2, got " + std::to_string(pic_width(f)) + "x" + std::to_string(pic_height(f));
+    return "";
+  }
+
+  void run(const std::vector<Elements>& windows, size_t i0, size_t i1, Elements& out) {
+    const i32 n = (i32)(i1 - i0);
+    const Frame* f0 = windows[i0][0].is_null() ? nullptr : windows[i0][0].as_const_frame();
+    std::string why = args_problem_;
+    for (size_t q = i0; q < i1 && why.empty(); ++q)
+      for (const Element& e : windows[q]) {
+        if (e.is_null()) {
+          why = "null input frame";
+          break;
+        }
+        why = frame_problem(e.as_const_frame());
+        if (why.empty() && (!f0 || !(e.as_const_frame()->as_frame_info() == f0->as_frame_info())))
+          why = "frames of one window differ in size";
+        if (!why.empty()) break;
+      }
+    if (!why.empty()) {
+      report_kernel_error("OpticalFlowTVL1, row " + std::to_string(windows[i0][0].index) + ": " + why);
+      for (i32 k = 0; k < n; ++k) out.push_back(Element());
+      return;
+    }
+    const int w = pic_width(f0), h = pic_height(f0);
+    const size_t px = (size_t)w * h;
+    // each distinct frame of the run once (the `next` of one window is the `prev` of the following one)
+    std::map<const u8*, int> slot;
+    std::vector<const u8*> distinct;
+    for (size_t q = i0; q < i1; ++q)
+      for (const Element& e : windows[q]) {
+        const u8* d = e.as_const_frame()->data;
+        if (slot.emplace(d, (int)distinct.size()).second) distinct.push_back(d);
+      }
+    const bool direct = !is_nv12(f0) && f0->channels() == 1;
+    std::vector<const u8*> gray(distinct.size());
+    if (direct) {
+      gray = distinct;
+    } else {
+      if (gray_bytes_ < px * distinct.size()) {
+        if (gray_) delete_buffer(device_, gray_);
+        gray_bytes_ = px * distinct.size();
+        gray_ = new_buffer(device_, gray_bytes_);
+      }
+      std::vector<u8*> dst(distinct.size());
+      for (size_t k = 0; k < distinct.size(); ++k) dst[k] = gray_ + k * px;
+      const int code = scn_convert_color_code("COLOR_RGB2GRAY");
+      if (is_nv12(f0)) {
+        std::vector<const u8*> chroma;
+        for (const u8* p : distinct) chroma.push_back(p + px);
+        SCN_CHECK(scn_convert_color_nv12(distinct.data(), chroma.data(), (size_t)w, (int)distinct.size(), w, h, code,
+                                         dst.data(), device_stream(device_)));
+      } else {
+        SCN_CHECK(scn_convert_color_u8(distinct.data(), (int)distinct.size(), w, h, code, dst.data(),
+                                       device_stream(device_)));
+      }
+      for (size_t k = 0; k < distinct.size(); ++k) gray[k] = dst[k];
+    }
+    const size_t need = scn_tvl1_workspace_bytes(w, h, n);
+    if (workspace_bytes_ < need) {
+      if (workspace_) delete_buffer(device_, workspace_);
+      workspace_bytes_ = need;
+      workspace_ = new_buffer(device_, need);
+    }
+    std::vector<Frame*> outs = new_frames(device_, FrameInfo(h, w, 2, FrameType::F32), n);
+    std::vector<const u8*> prev, next;
+    std::vector<float*> flow;
+    for (size_t q = i0; q < i1; ++q) {
+      prev.push_back(gray[slot[windows[q][0].as_const_frame()->data]]);
+      next.push_back(gray[slot[windows[q][1].as_const_frame()->data]]);
+      flow.push_back(reinterpret_cast<float*>(outs[q - i0]->data));
+    }
+    SCN_CHECK(call(prev.data(), next.data(), n, w, h, flow.data()));
+    for (i32 k = 0; k < n; ++k) insert_frame(out, outs[k]);
+  }
+
+  DeviceHandle device_;
+  std::string args_problem_;
+  float tau_ = 0.25f, lambda_ = 0.15f, theta_ = 0.3f, epsilon_ = 0.01f, scale_step_ = 0.8f;
+  int nscales_ = 5, warps_ = 5, iterations_ = 300, median_ = 5;
+  u8* workspace_ = nullptr;
+  size_t workspace_bytes_ = 0;
+  u8* gray_ = nullptr;  // gray copies of the batch's distinct RGB24 / NV12 frames
+  size_t gray_bytes_ = 0;
+};
+
+REGISTER_OP(OpticalFlowTVL1).frame_input("frame").frame_output("flow").stencil({0, 1}).protobuf_name(
+    "OpticalFlowTVL1Args");
+
+REGISTER_KERNEL(OpticalFlowTVL1, OpticalFlowTVL1KernelGPU)
+    .device(DeviceType::GPU)
+    .batch(8)
+    .num_devices(1)
+    .input_layout("frame", FrameLayout::NV12);
+
+// ---------------------------------------------------------------------------------------------
 // FrameDigest: frame -> 16 bytes (scn_frame_digest).  Lets frame-valued columns that are too large to
 // bring back (flow fields) be compared exactly between runs; not a reference op.
 class FrameDigestKernelGPU : public BatchedKernel {

@@ -394,3 +394,45 @@ def frame_digest(frames):
     pp, keep = cabi.ptr_array([frames.data_ptr() + i * nbytes for i in range(n)])
     cabi.check(cabi.lib().scn_frame_digest(pp, n, nbytes, out.data_ptr(), _stream()), "scn_frame_digest")
     return out
+
+
+def tvl1_workspace_bytes(width, height, n):
+    """Device scratch one scn_tvl1_u8 call of n pairs needs (reusable across calls on one stream)."""
+    return cabi.lib().scn_tvl1_workspace_bytes(width, height, n)
+
+
+def tvl1_flow(prev, next, tau=0.25, lambda_=0.15, theta=0.3, nscales=5, warps=5, epsilon=0.01, iterations=300,
+              scale_step=0.8, median_filtering=5, return_iterations=False, workspace=None):
+    """TV-L1 dense flow of n pairs (scn_tvl1_u8; DESIGN.md "TV-L1"): (N,H,W) gray or (N,H,W,3) RGB uint8 CUDA
+    tensors x2 -> (N,H,W,2) float32 (dx, dy).  RGB goes through convert_color(COLOR_RGB2GRAY) first.  epsilon <= 0
+    runs every warp for all `iterations`.  With return_iterations, also an int32 numpy array [N][nscales][warps]
+    of the iterations each (pair, level, warp) ran (level 0 = finest); the call then waits for the GPU."""
+    _need_cuda(prev, next)
+    grays = []
+    for t in (prev, next):
+        assert t.dtype == torch.uint8, t.dtype
+        if t.dim() == 4 and t.shape[3] == 3:
+            t = convert_color(t, "COLOR_RGB2GRAY")[..., 0]
+        elif t.dim() == 4 and t.shape[3] == 1:
+            t = t[..., 0]
+        if t.dim() != 3:
+            raise cabi.ScnError(f"tvl1_flow takes (N,H,W) gray or (N,H,W,3) RGB frames, got {tuple(t.shape)}")
+        grays.append(t.contiguous())
+    g0, g1 = grays
+    if g0.shape != g1.shape:
+        raise cabi.ScnError(f"tvl1_flow: prev {tuple(g0.shape)} and next {tuple(g1.shape)} differ")
+    n, h, w = g0.shape
+    out = torch.empty((n, h, w, 2), dtype=torch.float32, device=g0.device)
+    need = tvl1_workspace_bytes(w, h, n)
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(max(need, 1), dtype=torch.uint8, device=g0.device)
+    pp, k1 = cabi.ptr_array([g0.data_ptr() + i * h * w for i in range(n)])
+    np_, k2 = cabi.ptr_array([g1.data_ptr() + i * h * w for i in range(n)])
+    op, k3 = cabi.ptr_array([out.data_ptr() + i * h * w * 8 for i in range(n)])
+    iters = np.zeros((n, int(nscales), int(warps)), np.int32) if return_iterations else None
+    ip = iters.ctypes.data_as(ctypes.POINTER(ctypes.c_int)) if return_iterations else None
+    rc = cabi.lib().scn_tvl1_u8(pp, np_, n, w, h, op, tau, lambda_, theta, int(nscales), int(warps), epsilon,
+                                int(iterations), scale_step, int(median_filtering), ip, workspace.data_ptr(),
+                                workspace.numel(), _stream())
+    cabi.check(rc, "scn_tvl1_u8")
+    return (out, iters) if return_iterations else out
