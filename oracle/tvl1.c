@@ -105,12 +105,54 @@ int orc_tvl1_levels(int width, int height, int nscales, float scale_step, int* w
   return n;
 }
 
+/* lane 0 of a 32-lane __shfl_down_sync tree at offsets 16, 8, 4, 2, 1 (v is overwritten) */
+static float tv_lane_tree_f(float* v) {
+  for (int o = 16; o > 0; o >>= 1)
+    for (int l = 0; l < o; ++l) v[l] += v[l + o];
+  return v[0];
+}
+static double tv_lane_tree_d(double* v) {
+  for (int o = 16; o > 0; o >>= 1)
+    for (int l = 0; l < o; ++l) v[l] += v[l + o];
+  return v[0];
+}
+
+/* sum of term[0 .. npx) in tvl1_iterate_kernel's order.  Tile t is pixels [1024 t, 1024 t + 1024); thread x of
+ * 256 adds, in float from 0, the terms of pixels 1024 t + 256 j + x (j = 0..3, below npx); each warp of 32 threads
+ * is reduced by the lane tree, and the 8 warp sums are added in order from 0 in float.  The tile sums of one pair
+ * are then summed in double: thread x adds tiles x, x + 256, ... in order from 0, and the same lane tree and warp
+ * order reduce the 256 thread sums. */
+double orc_tvl1_tile_sum(const float* term, int npx) {
+  const int tiles = (npx + 1023) / 1024;
+  double acc[256];
+  for (int x = 0; x < 256; ++x) acc[x] = 0.0;
+  for (int t = 0; t < tiles; ++t) {
+    float e[256];
+    for (int x = 0; x < 256; ++x) {
+      e[x] = 0.f;
+      for (int j = 0; j < 4; ++j) {
+        const long i = 1024L * t + 256L * j + x;
+        if (i >= npx) break;
+        e[x] += term[i];
+      }
+    }
+    float s = 0.f;
+    for (int k = 0; k < 8; ++k) s += tv_lane_tree_f(e + 32 * k);
+    acc[t % 256] += (double)s;
+  }
+  double s = 0.0;
+  for (int k = 0; k < 8; ++k) s += tv_lane_tree_d(acc + 32 * k);
+  return s;
+}
+
 /* gray0, gray1: u8 [height][width] -> flow float32 [height][width][2] = (dx, dy).  iters (nullable):
  * int [nscales][warps], level 0 (finest) first, the iterations each (level, warp) ran; 0 for levels the pyramid
- * does not have.  Arguments are assumed valid (kernels.py / tests check them). */
+ * does not have.  tile_error = 0 sums the stop error sequentially in double (the specification); 1 sums the same
+ * float terms as tvl1_iterate_kernel does (orc_tvl1_tile_sum), so that the stop decisions match the kernel's.
+ * Arguments are assumed valid (kernels.py / tests check them). */
 void orc_tvl1_u8(const uint8_t* gray0, const uint8_t* gray1, int width, int height, float tau, float lambda,
                  float theta, int nscales, int warps, float epsilon, int iterations, float scale_step,
-                 int median_filtering, float* flow, int* iters) {
+                 int median_filtering, int tile_error, float* flow, int* iters) {
   int lw[16], lh[16];
   const int L = orc_tvl1_levels(width, height, nscales, scale_step, lw, lh);
   if (iters) memset(iters, 0, sizeof(int) * (size_t)nscales * warps);
@@ -133,6 +175,7 @@ void orc_tvl1_u8(const uint8_t* gray0, const uint8_t* gray1, int width, int heig
   float *u1 = buf[0], *u2 = buf[1], *c1 = buf[2], *c2 = buf[3], *Ix = buf[4], *Iy = buf[5], *wx = buf[6],
         *wy = buf[7], *rho_c = buf[8], *p11 = buf[9], *p12 = buf[10], *p21 = buf[11], *p22 = buf[12];
   float* tmp = (float*)malloc(sizeof(float) * px0);
+  float* term = tile_error ? (float*)malloc(sizeof(float) * px0) : NULL;
   const float l_t = lambda * theta, taut = tau / theta;
   const double eps2 = epsilon > 0.f ? (double)epsilon * epsilon : -1.0;
   const float up = (float)(1.0 / scale_step);
@@ -203,10 +246,15 @@ void orc_tvl1_u8(const uint8_t* gray0, const uint8_t* gray1, int width, int heig
             const float div2 = (p21[i] - (x > 0 ? p21[i - 1] : 0.f)) + (p22[i] - (y > 0 ? p22[i - w] : 0.f));
             const float n1 = v1 + theta * div1, n2 = v2 + theta * div2;
             const float e1 = n1 - u1[i], e2 = n2 - u2[i];
-            acc += (double)(e1 * e1 + e2 * e2);
+            const float e = e1 * e1 + e2 * e2;
+            if (term)
+              term[i] = e;
+            else
+              acc += (double)e;
             u1[i] = n1;
             u2[i] = n2;
           }
+        if (term) acc = orc_tvl1_tile_sum(term, (int)npx);
         error = acc / (double)npx;
         for (int y = 0; y < h; ++y)
           for (int x = 0; x < w; ++x) {
@@ -236,6 +284,7 @@ void orc_tvl1_u8(const uint8_t* gray0, const uint8_t* gray1, int width, int heig
     flow[2 * i + 1] = u2[i];
   }
   free(tmp);
+  free(term);
   for (int b = 0; b < 13; ++b) free(buf[b]);
   for (int s = 0; s < L; ++s) {
     free(I0[s]);

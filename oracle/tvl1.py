@@ -84,10 +84,21 @@ def median(img, k):
     return out
 
 
-def flow(frame0, frame1, return_iterations=False, **params):
+def tile_sum(terms):
+    """The sum of float32 terms in the order of tvl1_iterate_kernel's stop error (orc_tvl1_tile_sum), as a float."""
+    terms = np.ascontiguousarray(terms, np.float32).ravel()
+    L = lib()
+    L.orc_tvl1_tile_sum.restype = ctypes.c_double
+    return L.orc_tvl1_tile_sum(_p(terms), int(terms.size))
+
+
+def flow(frame0, frame1, return_iterations=False, error_sum="sequential", **params):
     """TV-L1 dense flow of one pair -> (H, W, 2) float32 (dx, dy).  Frames are u8 gray (H, W) or RGB (H, W, 3).
     Keyword parameters as DEFAULTS.  With return_iterations, also int32 [nscales][warps]: the iterations each
-    (level, warp) ran, level 0 (finest) first, 0 for levels the pyramid stops before."""
+    (level, warp) ran, level 0 (finest) first, 0 for levels the pyramid stops before.  error_sum: "sequential"
+    sums the stop error in double pixel by pixel (the specification); "tiles" sums the same float terms in the
+    order of the GPU kernel (tile_sum), so that a warp step stops after the same iteration as on the GPU."""
+    assert error_sum in ("sequential", "tiles"), error_sum
     p = dict(DEFAULTS)
     unknown = set(params) - set(p)
     assert not unknown, unknown
@@ -100,7 +111,7 @@ def flow(frame0, frame1, return_iterations=False, **params):
     f = ctypes.c_float
     lib().orc_tvl1_u8(_p(g0), _p(g1), w, h, f(p["tau"]), f(p["lambda_"]), f(p["theta"]), int(p["nscales"]),
                       int(p["warps"]), f(p["epsilon"]), int(p["iterations"]), f(p["scale_step"]),
-                      int(p["median_filtering"]), _p(out), _p(iters))
+                      int(p["median_filtering"]), int(error_sum == "tiles"), _p(out), _p(iters))
     return (out, iters) if return_iterations else out
 
 
