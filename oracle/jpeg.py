@@ -165,11 +165,15 @@ def _fdct_1d(d, pass1):
     return out
 
 
+def fdct(blk):
+    """(..., 8, 8) samples -> (..., 8, 8) jpeg_fdct_islow of samples - 128 (8 times the orthonormal DCT)."""
+    d = _fdct_1d(blk.astype(np.int64) - 128, True)
+    return _fdct_1d(d.swapaxes(-1, -2), False).swapaxes(-1, -2)
+
+
 def fdct_quant(blk, qtab):
     """(..., 8, 8) samples -> (..., 64) quantised coefficients in zig-zag order."""
-    d = blk.astype(np.int64) - 128
-    d = _fdct_1d(d, True)
-    d = _fdct_1d(d.swapaxes(-1, -2), False).swapaxes(-1, -2)
+    d = fdct(blk)
     c = d.reshape(d.shape[:-2] + (64,))[..., ZIGZAG]
     q = 8 * qtab[ZIGZAG]
     return np.sign(c) * ((np.abs(c) + (q >> 1)) // q)
@@ -184,9 +188,10 @@ def _nbits(v):
     return n
 
 
-def entropy_code(coefs, comps, dc_luts, ac_luts):
+def _coded(coefs, comps, dc_luts, ac_luts):
     """coefs (nblocks, 64) in coding order; comps[i] = component of block i (DC predictor and table:
-    0 -> luma tables, else chroma) -> the scan's bytes, 1-padded and 0x00-stuffed."""
+    0 -> luma tables, else chroma) -> (the scan's bytes before stuffing, 1-padded; the symbols coded as an
+    (nsymbols, 3) array of (class 0 DC / 1 AC, table 0 luma / 1 chroma, symbol))."""
     nb = coefs.shape[0]
     dc = coefs[:, 0]
     prev = np.zeros(nb, np.int64)
@@ -194,21 +199,22 @@ def entropy_code(coefs, comps, dc_luts, ac_luts):
         idx = np.nonzero(comps == c)[0]
         prev[idx[1:]] = dc[idx[:-1]]
     tab = (comps != 0).astype(np.int64)
-    keys, vals, lens = [], [], []
+    keys, vals, lens, syms = [], [], [], []
 
-    def sym(key, lut_code, lut_size, s, v, nbits):
+    def sym(key, lut_code, lut_size, s, v, nbits, cls, t):
         # a Huffman symbol followed by nbits extra bits: negative values send v - 1 in nbits bits
         extra = np.where(v < 0, v - 1, v) & ((1 << nbits) - 1)
         keys.append(key)
         vals.append((lut_code[s] << nbits) | extra)
         lens.append(lut_size[s] + nbits)
+        syms.append(np.stack(np.broadcast_arrays(cls, t, s), -1).reshape(-1, 3))
 
     diff = dc - prev
     n = _nbits(diff)
     bidx = np.arange(nb, dtype=np.int64)
     for t in (0, 1):
         m = tab == t
-        sym(bidx[m] * 1024, *dc_luts[t], n[m], diff[m], n[m])
+        sym(bidx[m] * 1024, *dc_luts[t], n[m], diff[m], n[m], 0, t)
     blk, k = np.nonzero(coefs[:, 1:])
     k = k + 1
     v = coefs[blk, k]
@@ -223,14 +229,14 @@ def entropy_code(coefs, comps, dc_luts, ac_luts):
         for j in range(3):  # ZRL (0xF0) for every full 16 zeros of the run
             z = m & (run >> 4 > j)
             zero = np.zeros(z.sum(), np.int64)
-            sym(blk[z] * 1024 + k[z] * 8 + j, code, size, np.full(z.sum(), 0xF0), zero, zero)
-        sym(blk[m] * 1024 + k[m] * 8 + 4, code, size, ((run[m] & 15) << 4) | nz[m], v[m], nz[m])
+            sym(blk[z] * 1024 + k[z] * 8 + j, code, size, np.full(z.sum(), 0xF0), zero, zero, 1, t)
+        sym(blk[m] * 1024 + k[m] * 8 + 4, code, size, ((run[m] & 15) << 4) | nz[m], v[m], nz[m], 1, t)
     last = np.zeros(nb, np.int64)
     last[blk] = k  # the last nonzero index of each block (k increases within a block)
     for t in (0, 1):
         e = (last < 63) & (tab == t)
         zero = np.zeros(e.sum(), np.int64)
-        sym(bidx[e] * 1024 + 1000, *ac_luts[t], zero, zero, zero)
+        sym(bidx[e] * 1024 + 1000, *ac_luts[t], zero, zero, zero, 1, t)
     keys, vals, lens = (np.concatenate(a) for a in (keys, vals, lens))
     o = np.argsort(keys, kind="stable")
     vals, lens = vals[o], lens[o]
@@ -242,9 +248,19 @@ def entropy_code(coefs, comps, dc_luts, ac_luts):
     for j in range(int(lens.max()) if len(lens) else 0):
         m = lens > j
         bits[starts[m] + j] = (vals[m] >> (lens[m] - 1 - j)) & 1
-    data = np.packbits(bits)
-    ff = np.nonzero(data == 0xFF)[0]
-    return np.insert(data, ff + 1, 0).tobytes()
+    return np.packbits(bits), np.concatenate(syms)
+
+
+def stuff(data):
+    """a 0x00 after every 0xFF of the scan"""
+    data = np.frombuffer(bytes(data), np.uint8)
+    return np.insert(data, np.nonzero(data == 0xFF)[0] + 1, 0).tobytes()
+
+
+def entropy_code(coefs, comps, dc_luts, ac_luts):
+    """coefs (nblocks, 64) in coding order; comps[i] = component of block i (DC predictor and table:
+    0 -> luma tables, else chroma) -> the scan's bytes, 1-padded and 0x00-stuffed."""
+    return stuff(_coded(coefs, comps, dc_luts, ac_luts)[0])
 
 
 def _marker(m, payload):
@@ -273,9 +289,8 @@ def header(width, height, channels, quality):
     return out
 
 
-def encode(frame, quality=95):
-    """frame: (H, W, 3) RGB or (H, W) / (H, W, 1) gray uint8 -> the bytes of
-    cv2.imencode('.jpg', frame[..., ::-1] (or the gray frame), [cv2.IMWRITE_JPEG_QUALITY, quality])."""
+def _blocks_in_order(frame, quality):
+    """-> (width, height, channels, coefficients in coding order, component of each block, Huffman lookups)"""
     frame = np.asarray(frame, np.uint8)
     if frame.ndim == 3 and frame.shape[2] == 1:
         frame = frame[..., 0]
@@ -308,7 +323,29 @@ def encode(frame, quality=95):
         crq = fdct_quant(blocks(downsample(cr, 8 * mh, 8 * mw)), cq)
         coefs = np.concatenate([mcu, cbq[:, :, None], crq[:, :, None]], axis=2).reshape(-1, 64)
         comps = np.tile(np.array([0, 0, 0, 0, 1, 2]), mh * mw)
+    return w, h, channels, coefs, comps, luts
+
+
+def encode(frame, quality=95):
+    """frame: (H, W, 3) RGB or (H, W) / (H, W, 1) gray uint8 -> the bytes of
+    cv2.imencode('.jpg', frame[..., ::-1] (or the gray frame), [cv2.IMWRITE_JPEG_QUALITY, quality])."""
+    w, h, channels, coefs, comps, luts = _blocks_in_order(frame, quality)
     return header(w, h, channels, quality) + entropy_code(coefs, comps, *luts) + b"\xFF\xD9"
+
+
+def scan(frame, quality=95):
+    """The entropy-coded segment of encode(frame, quality) before stuffing: the 1-padded bit stream, whose bytes
+    the encoder's 0xFF passes split into chunks."""
+    _, _, _, coefs, comps, luts = _blocks_in_order(frame, quality)
+    return _coded(coefs, comps, *luts)[0].tobytes()
+
+
+def symbols(frame, quality=95):
+    """{(class, table, symbol): count} of the Huffman symbols encode(frame, quality) codes: class 0 DC (symbol the
+    category 0-11) or 1 AC (symbol run << 4 | size, 0x00 EOB, 0xF0 ZRL); table 0 luma or 1 chroma."""
+    _, _, _, coefs, comps, luts = _blocks_in_order(frame, quality)
+    keys, counts = np.unique(_coded(coefs, comps, *luts)[1], axis=0, return_counts=True)
+    return {tuple(int(x) for x in k): int(c) for k, c in zip(keys, counts)}
 
 
 # ---- the sweep the tests hold encoders to -------------------------------------------------------------------------
@@ -348,6 +385,29 @@ def sweep():
             for h, w, channels in ((17, 31, 3), (33, 19, 1)):
                 cases.append((f"{kind}_{h}x{w}x{channels}_q{q}", content(kind, h, w, channels, q), q))
     return cases
+
+
+# every Huffman symbol a table can code: DC categories 0-11; AC (run, size) for runs 0-15 and sizes 1-10, EOB, ZRL
+DC_SYMBOLS = tuple(range(12))
+AC_SYMBOLS = tuple(sorted({(r << 4) | s for r in range(16) for s in range(1, 11)} | {0x00, 0xF0}))
+
+
+def symbol_corpus_frames(corpus):
+    """The frames of tests/golden/jpeg_symbols.npz (oracle/make_golden_jpeg_symbols.py) -> [(name, frame, quality)].
+    Key "luma_q<Q>" holds 8 x 8 blocks laid side by side in a gray 8 x 8n frame, coded in that order.  Key
+    "chroma_q<Q>" holds 8 x 8 blocks X, each doubled to a 16 x 16 MCU of pixels (255 - X, 255 - X, X), whose
+    Cb is X exactly; the MCUs lie side by side in a 16 x 16n RGB frame."""
+    out = []
+    for key in sorted(corpus.keys(), key=lambda k: (k.split("_")[0], -int(k.split("_q")[1]))):
+        table, q = key.split("_q")
+        b = np.asarray(corpus[key], np.uint8)
+        if table == "luma":
+            frame = np.ascontiguousarray(b.transpose(1, 0, 2).reshape(8, -1))
+        else:
+            x = b.repeat(2, 1).repeat(2, 2).transpose(1, 0, 2).reshape(16, -1)
+            frame = np.ascontiguousarray(np.stack([255 - x, 255 - x, x], -1))
+        out.append((key, frame, int(q)))
+    return out
 
 
 def cv2_encode(frame, quality):
