@@ -7,9 +7,12 @@
 //   R_i   = polynomial expansion (separable (2n+1)-tap Gaussian-weighted basis, 5 coefficients)
 //   M     = UpdateMatrices(R0, R1 warped by the current flow)        (5 floats per pixel)
 //   flow  = solve 2x2 from the winSize x winSize box average of M,   numIters times
-// Floating point: sums are taken in a different order than OpenCV's SIMD code, so parity is within
-// a tolerance (tests/test_flow_gpu.py), not bit-exact.  The 2x2 solve runs in double like OpenCV's (the
-// determinant cancels catastrophically in float); the window sums in float (box_solve_f32_kernel) or double.
+// Floating point: sums are taken in a different order than OpenCV's SIMD code, so parity with cv2 is within a
+// tolerance (tests/test_flow_gpu.py).  Every rounding is written out (explicit __fmaf_rn / __fma_rn wherever a product
+// is fused; flow.o is built with -fmad=false so that nvcc contracts nothing on its own), and the kernel-ordered C
+// restatement oracle/farneback_k.c evaluates the same expressions in the same order: the kernels equal it bit for bit
+// (tests/test_flow_exact_gpu.py).  The 2x2 solve runs in double like OpenCV's (the determinant cancels
+// catastrophically in float); the window sums in float (box_solve_f32_kernel) or double.
 // All kernels are plain per-pixel / separable memory-bound passes (no tensor cores).
 #include <math.h>
 #include <stdlib.h>
@@ -164,11 +167,16 @@ __global__ void update_matrices_kernel(const float* __restrict__ R0, const float
     const float a00 = (1.f - fx) * (1.f - fy), a01 = fx * (1.f - fy), a10 = (1.f - fx) * fy, a11 = fx * fy;
     const float* p = R1 + (size_t)y1 * w + x1;
     const float* q = p + w;
-    r2 = a00 * p[0] + a01 * p[1] + a10 * q[0] + a11 * q[1];
-    r3 = a00 * p[ps] + a01 * p[ps + 1] + a10 * q[ps] + a11 * q[ps + 1];
-    r4 = a00 * p[2 * ps] + a01 * p[2 * ps + 1] + a10 * q[2 * ps] + a11 * q[2 * ps + 1];
-    r5 = a00 * p[3 * ps] + a01 * p[3 * ps + 1] + a10 * q[3 * ps] + a11 * q[3 * ps + 1];
-    r6 = a00 * p[4 * ps] + a01 * p[4 * ps + 1] + a10 * q[4 * ps] + a11 * q[4 * ps + 1];
+    // per plane: a01 p[1] rounded, then the a00, a10 and a11 taps fused in that order
+    float rr[5];
+#pragma unroll
+    for (int c = 0; c < 5; ++c) {
+      const float p0 = p[c * ps], p1 = p[c * ps + 1];
+      float t = __fmaf_rn(a00, p0, a01 * p1);
+      t = __fmaf_rn(a10, q[c * ps], t);
+      rr[c] = __fmaf_rn(a11, q[c * ps + 1], t);
+    }
+    r2 = rr[0], r3 = rr[1], r4 = rr[2], r5 = rr[3], r6 = rr[4];
     r4 = (r0[2] + r4) * 0.5f;
     r5 = (r0[3] + r5) * 0.5f;
     r6 = (r0[4] + r6) * 0.25f;
@@ -178,10 +186,10 @@ __global__ void update_matrices_kernel(const float* __restrict__ R0, const float
     r5 = r0[3];
     r6 = r0[4] * 0.5f;
   }
-  r2 = (r0[0] - r2) * 0.5f;
-  r3 = (r0[1] - r3) * 0.5f;
-  r2 += r4 * dy + r6 * dx;
-  r3 += r6 * dy + r5 * dx;
+  r2 = r0[0] - r2;
+  r3 = r0[1] - r3;
+  r2 = __fmaf_rn(r2, 0.5f, __fmaf_rn(dy, r4, dx * r6));  // (r0 - r2) / 2 + r4 dy + r6 dx
+  r3 = __fmaf_rn(r3, 0.5f, __fmaf_rn(dx, r5, dy * r6));  // (r0 - r3) / 2 + r6 dy + r5 dx
   if ((unsigned)(x - BORDER) >= (unsigned)(w - BORDER * 2) || (unsigned)(y - BORDER) >= (unsigned)(h - BORDER * 2)) {
     const float scale = (x < BORDER ? border[x] : 1.f) * (x >= w - BORDER ? border[w - x - 1] : 1.f) *
                         (y < BORDER ? border[y] : 1.f) * (y >= h - BORDER ? border[h - y - 1] : 1.f);
@@ -192,11 +200,19 @@ __global__ void update_matrices_kernel(const float* __restrict__ R0, const float
     r6 *= scale;
   }
   float* m = M + (size_t)y * w + x;
-  m[0] = r4 * r4 + r6 * r6;
+  m[0] = __fmaf_rn(r4, r4, r6 * r6);
   m[ps] = (r4 + r5) * r6;
-  m[2 * ps] = r5 * r5 + r6 * r6;
-  m[3 * ps] = r4 * r2 + r6 * r3;
-  m[4 * ps] = r6 * r2 + r5 * r3;
+  m[2 * ps] = __fmaf_rn(r5, r5, r6 * r6);
+  m[3 * ps] = __fmaf_rn(r2, r4, r3 * r6);
+  m[4 * ps] = __fmaf_rn(r3, r5, r2 * r6);
+}
+
+// the 2x2 solve of FarnebackUpdateFlow_Blur in double: each difference of products rounds the subtracted product and
+// fuses the other, (g11 g22 - g12^2 + 1e-3) is inverted once, the flow rounded to float last
+__device__ __forceinline__ float2 solve2x2(double g11, double g12, double g22, double h1, double h2) {
+  const double idet = 1. / (__fma_rn(g11, g22, -__dmul_rn(g12, g12)) + 1e-3);
+  return make_float2((float)(__fma_rn(g11, h2, -__dmul_rn(g12, h1)) * idet),
+                     (float)(__fma_rn(g22, h1, -__dmul_rn(g12, h2)) * idet));
 }
 
 // box filter, vertical pass in double (rows clamped); one thread per (x, channel)
@@ -224,9 +240,9 @@ __global__ void box_h_solve_kernel(const double* __restrict__ V, int w, int h, i
     for (int c = 0; c < 5; ++c) hs[c] += p[c * ps];
   }
   const double g11 = hs[0] * scale, g12 = hs[1] * scale, g22 = hs[2] * scale, h1 = hs[3] * scale, h2 = hs[4] * scale;
-  const double idet = 1. / (g11 * g22 - g12 * g12 + 1e-3);
-  flow[((size_t)y * w + x) * 2] = (float)((g11 * h2 - g12 * h1) * idet);
-  flow[((size_t)y * w + x) * 2 + 1] = (float)((g22 * h1 - g12 * h2) * idet);
+  const float2 f = solve2x2(g11, g12, g22, h1, h2);
+  flow[((size_t)y * w + x) * 2] = f.x;
+  flow[((size_t)y * w + x) * 2 + 1] = f.y;
 }
 
 
@@ -441,9 +457,9 @@ box_solve_fused_kernel(const float* __restrict__ M, int w, int h, double scale, 
     if (x >= w) break;
     const double g11 = hs[o][0] * scale, g12 = hs[o][1] * scale, g22 = hs[o][2] * scale, h1 = hs[o][3] * scale,
                  h2 = hs[o][4] * scale;
-    const double idet = 1. / (g11 * g22 - g12 * g12 + 1e-3);
-    flow[((size_t)y * w + x) * 2] = (float)((g11 * h2 - g12 * h1) * idet);
-    flow[((size_t)y * w + x) * 2 + 1] = (float)((g22 * h1 - g12 * h2) * idet);
+    const float2 f = solve2x2(g11, g12, g22, h1, h2);
+    flow[((size_t)y * w + x) * 2] = f.x;
+    flow[((size_t)y * w + x) * 2 + 1] = f.y;
   }
 }
 
@@ -537,8 +553,7 @@ box_solve_f32_kernel(const float* __restrict__ M, int w, int h, double scale, fl
     for (int o = 0; o < 4; ++o) {
       const double g11 = hs[o][0] * scale, g12 = hs[o][1] * scale, g22 = hs[o][2] * scale, h1 = hs[o][3] * scale,
                    h2 = hs[o][4] * scale;
-      const double idet = 1. / (g11 * g22 - g12 * g12 + 1e-3);
-      out[o] = make_float2((float)((g11 * h2 - g12 * h1) * idet), (float)((g22 * h1 - g12 * h2) * idet));
+      out[o] = solve2x2(g11, g12, g22, h1, h2);
     }
     float2* dst = reinterpret_cast<float2*>(flow) + (size_t)y * w + x0 + gx * 4;
 #pragma unroll

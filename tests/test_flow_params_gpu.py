@@ -3,9 +3,9 @@
 tests/test_flow_gpu.py holds the kernels at the reference's arguments (3, 0.5, 15, 3, 5, 1.2).  scn_farneback_u8c3
 accepts more, and several code paths run only off those defaults: the generic-radius Gaussian, the generic-poly_n
 expansion, the double two-pass box for win_size != 15, the per-level expansion without the pyramid cache, 2 or 4
-pyramid levels, a single iteration.  The oracle is held to cv2 over the same arguments by
-tests/test_flow_params_cpu.py, so it is the reference here.  Bounds are those of test_flow_gpu.py: max |d| <= 2e-3
-px and mean |d| <= 1e-4 px on smooth motion."""
+pyramid levels, a single iteration.  The reference here is the kernel-ordered oracle (oracle/farneback_k.c), held
+to orc_farneback_u8 -- and through it to cv2 -- over the same arguments by tests/test_flow_exact_cpu.py and
+tests/test_flow_params_cpu.py; the kernels equal it bit for bit.  The 1080p num_levels=4 case is also held to cv2."""
 import ctypes
 import os
 import subprocess
@@ -16,16 +16,17 @@ import numpy as np
 import pytest
 import torch
 
-import oracle
+from oracle import farneback_k
 from oracle import synth
 from scanner_b200 import cabi, kernels, protolite
 from scanner_b200 import engine as E
+
+from helpers.flow_cases import DEFAULTS, EDGES, GRID
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SCN_E_BADARG, SCN_E_UNSUPPORTED = -1, -2
-DEFAULTS = dict(num_levels=3, pyr_scale=0.5, win_size=15, num_iters=3, poly_n=5, poly_sigma=1.2)
 
 
 def dev(a):
@@ -53,48 +54,22 @@ def _check(got, want, what, max_d=2e-3, outliers=0):
     assert d.max() <= max_d and d.mean() <= 1e-4 and n_out <= outliers, (what, d.max(), d.mean(), n_out)
 
 
-def _vs_oracle(h, w, over, seed, **bound):
+def _vs_oracle(h, w, over, seed):
     a = dict(DEFAULTS, **over)
     f0, f1 = synth.flow_pair(seed, h, w, "shift")
     got, ran = _ran(lambda: kernels.optical_flow(dev(f0[None]), dev(f1[None]), **a)[0].cpu().numpy())
-    want = oracle.farneback(oracle.bgr2gray(f0), oracle.bgr2gray(f1), **a)
-    _check(got, want, f"{h}x{w} {over}", **bound)
+    want = farneback_k.flow(f0, f1, **a)
+    assert np.array_equal(got, want), (h, w, over, float(np.abs(got - want).max()))
     return ran
 
 
 # ---- a. the argument grid against the oracle ------------------------------------------------------------------------
-GRID = [
-    (540, 960, dict(num_levels=4)),                          # Gaussian radius 19: gauss_fused_kernel<0>; 4 levels
-    (270, 480, dict(pyr_scale=0.7)),                         # radius 2 at level 3: gauss_fused_kernel<0>
-    (96, 128, dict(pyr_scale=0.3)),
-    (270, 480, dict(poly_n=7, poly_sigma=1.5)),              # poly_fused_kernel<0>
-    (270, 480, dict(poly_n=3, poly_sigma=0.9)),
-    (96, 128, dict(poly_n=1, poly_sigma=0.6)),
-    (270, 480, dict(win_size=2)),                            # box_v_kernel + box_h_solve_kernel (double); bound below
-    (96, 128, dict(win_size=3)),
-    (96, 128, dict(win_size=4)),
-    (270, 480, dict(win_size=9)),
-    (96, 128, dict(win_size=16)),
-    (270, 480, dict(win_size=21)),
-    (270, 480, dict(pyr_scale=0.8, num_levels=8)),           # pyramid over 2 W H pixels: per-level expansion
-    (540, 960, dict(pyr_scale=0.7, num_levels=8, poly_n=7, poly_sigma=1.5)),
-    (540, 960, dict(pyr_scale=0.8, num_levels=8)),
-    (270, 480, dict(num_iters=1)),                           # no update_matrices_kernel between iterations
-    (96, 128, dict(num_iters=6)),
-    (96, 128, dict(num_levels=0)),
-]
 
 
 @pytest.mark.parametrize("h,w,over", GRID, ids=[f"{h}x{w}-" + "-".join(f"{k}{v}" for k, v in o.items())
                                                 for h, w, o in GRID])
 def test_kernels_match_the_oracle_off_the_default_arguments(h, w, over):
-    bound = {}
-    if over == dict(win_size=2):
-        # A 3 x 3 window (at scale 1/4) leaves ill-conditioned 2x2 systems: the worst pixel's flow is (11.6, -13.2) px
-        # where the motion is (1.5, -0.75), and there cv2 and the oracle already differ by 2.1e-2 px.  Measured on an
-        # H100: max 7.3e-2, mean 1.1e-5, 59 of 129600 pixels over 2e-3; the same with SCN_FLOW_BOX=f64 and unfused.
-        bound = dict(max_d=0.1, outliers=130)
-    ran = _vs_oracle(h, w, over, 2000 + h + w, **bound)
+    ran = _vs_oracle(h, w, over, 2000 + h + w)
     if over.get("win_size", 15) != 15:   # the f32 box kernel is instantiated for win_size 15 only
         assert ran.get("flow_box_v_kernel", 0) > 0 and ran.get("flow_box_h_solve_kernel", 0) > 0, ran
         assert "flow_box_solve_f32_kernel" not in ran, ran
@@ -124,8 +99,7 @@ def test_pyramid_cache_and_per_level_expansion_give_the_same_bits(monkeypatch):
     assert k_cached == 4 * n and k_plain == 2 * 4 * (n - 1), (k_cached, k_plain)
     assert torch.equal(cached, plain)
     for i in (0, n - 2):
-        want = oracle.optical_flow(frames[i], frames[i + 1])
-        assert np.abs(cached[i].cpu().numpy() - want).max() <= 2e-3, i
+        assert np.array_equal(cached[i].cpu().numpy(), farneback_k.flow(frames[i], frames[i + 1])), i
 
 
 def test_tiny_frames_take_the_per_level_expansion(monkeypatch):
@@ -136,14 +110,10 @@ def test_tiny_frames_take_the_per_level_expansion(monkeypatch):
     got, ran = _ran(lambda: kernels.optical_flow_sequence(dev(frames)))
     assert ran.get("flow_poly_fused_kernel", 0) == 2 * (n - 1), ran
     for i in range(n - 1):
-        assert np.abs(got[i].cpu().numpy() - oracle.optical_flow(frames[i], frames[i + 1])).max() <= 2e-3, i
+        assert np.array_equal(got[i].cpu().numpy(), farneback_k.flow(frames[i], frames[i + 1])), i
 
 
 # ---- b. edge geometries at the default arguments --------------------------------------------------------------------
-# frames smaller than the window; widths and heights at the tiles' edges (f32 box 88 x 32, Gaussian and polynomial
-# 64 x 32, update_matrices_kernel 32 x 8); 200 x 300 has two pyramid levels
-EDGES = [(1, 1), (2, 2), (1, 64), (64, 1), (4, 4), (14, 14),
-         (31, 87), (32, 88), (33, 89), (33, 87), (31, 89), (32, 64), (200, 300)]
 
 
 @pytest.mark.parametrize("h,w", EDGES, ids=[f"{h}x{w}" for h, w in EDGES])
