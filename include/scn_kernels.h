@@ -98,6 +98,9 @@ SCN_API int scn_resize_bilinear_u8c3_strided(const uint8_t* src, size_t src_stri
  *        BlurArgs.kernel_size, interior pixels only; sigma is unused by the reference).
  * Border pixels (which the reference leaves uninitialised) are written as 0.
  * kernel_size in [1, 31].  Bit-exact on the interior.
+ * Limits, checked before any launch: width in [1, 2^29] (row offsets are int arithmetic) and
+ * kernel_size outside [1, 31] return SCN_E_BADARG; a frame taller than 2,097,120 rows (65,535
+ * tiles of 32 rows in the grid's y dimension) returns SCN_E_UNSUPPORTED.
  */
 SCN_API int scn_box_blur_u8c3(const uint8_t* const* host_src_ptrs, int n, int width, int height,
                       int kernel_size, uint8_t* const* host_dst_ptrs, void* stream);

@@ -74,6 +74,28 @@ def blur(frame, kernel_size):
     return out
 
 
+def blur_sat(frame, kernel_size):
+    """blur() restated with a summed-area table, O(1) per sample: fl = ceil(k/2) - 1, fr = k/2; an interior sample
+    is the sum of its (fl + fr + 1)^2 window integer-divided by (fl + fr + 1)^2, every other sample is 0 (so is the
+    whole frame when a side is shorter than the window).  Sums are uint32 with wrap-around: a window sum is below
+    31^2 * 255 < 2^32, so differences of wrapped prefix sums are exact.  Takes (H, W, 3) or (N, H, W, 3)."""
+    frame = np.asarray(frame, dtype=np.uint8)
+    h, w = frame.shape[-3], frame.shape[-2]
+    fl, fr = (kernel_size + 1) // 2 - 1, kernel_size // 2
+    k = fl + fr + 1
+    out = np.zeros_like(frame)
+    if h < k or w < k:
+        return out
+    s = np.zeros(frame.shape[:-3] + (h + 1, w + 1, frame.shape[-1]), np.uint32)
+    np.cumsum(frame, axis=-3, dtype=np.uint32, out=s[..., 1:, 1:, :])
+    np.cumsum(s[..., 1:, 1:, :], axis=-2, dtype=np.uint32, out=s[..., 1:, 1:, :])
+    win = s[..., k:, k:, :] - s[..., :-k, k:, :]
+    win -= s[..., k:, :-k, :]
+    win += s[..., :-k, :-k, :]
+    out[..., fl:h - fr, fl:w - fr, :] = win // np.uint32(k * k)
+    return out
+
+
 def blur_interior(h, w, kernel_size):
     """Slices of the region the reference actually writes (test_ops.cpp:278-279)."""
     import math

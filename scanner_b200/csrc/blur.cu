@@ -322,7 +322,9 @@ box_packed_kernel(PtrBatch src, MutPtrBatch dst, int width, int height, int rows
 
 int launch_blur(const uint8_t* const* sp, int n, int width, int height, int ksize,
                 uint8_t* const* dp, cudaStream_t st) {
-  if (n < 0 || width <= 0 || height <= 0 || ksize < 1 || ksize > KMAX) return SCN_E_BADARG;
+  // byte offsets within a row reach width * 3 plus a tile's halo in int arithmetic: 2^29 pixels keep them far
+  // from INT_MAX
+  if (n < 0 || width <= 0 || width > (1 << 29) || height <= 0 || ksize < 1 || ksize > KMAX) return SCN_E_BADARG;
   if (n == 0) return 0;
   if (!sp || !dp) return SCN_E_BADARG;
   const int fl = (ksize + 1) / 2 - 1;  // ceil(k/2.0) - 1
@@ -330,7 +332,9 @@ int launch_blur(const uint8_t* const* sp, int n, int width, int height, int ksiz
   const int k = fl + fr + 1;
   const int in_w = TW + k - 1, in_h = TH + k - 1;
   const size_t smem = (((size_t)in_h * in_w * 3 + 15) & ~(size_t)15) + (size_t)in_h * TW * 3 * 2;
-  if (((height + TH - 1) / TH) > 65535) return SCN_E_UNSUPPORTED;
+  // box_generic_kernel's grid has one y block per TH rows (at most 65535); past this bound no row count is
+  // rounded up in int arithmetic either
+  if (height > 65535 * TH) return SCN_E_UNSUPPORTED;
   return for_each_chunk(n, [&](int i0, int cnt) {
     const PtrBatch s = gather<PtrBatch>(sp, i0, cnt);
     const MutPtrBatch d = gather<MutPtrBatch>(dp, i0, cnt);
@@ -383,8 +387,8 @@ extern "C" int scn_box_blur_u8c3(const uint8_t* const* host_src_ptrs, int n, int
 extern "C" int scn_box_blur_u8c3_strided(const uint8_t* src, size_t stride_bytes, int n,
                                          int width, int height, int kernel_size, uint8_t* dst,
                                          void* stream) {
-  if (n < 0) return SCN_E_BADARG;
-  if (n == 0) return 0;
+  // n <= 0: the same argument checks as the pointer-list entry, no launch
+  if (n <= 0) return scn::launch_blur(nullptr, n, width, height, kernel_size, nullptr, (cudaStream_t)stream);
   if (!src || !dst) return SCN_E_BADARG;
   return scn::launch_blur(scn::strided(src, stride_bytes, n).data(), n, width, height, kernel_size,
                           scn::strided(dst, stride_bytes, n).data(), (cudaStream_t)stream);

@@ -502,9 +502,15 @@ class HistogramKernelCPU : public BatchedKernel {
     u8* block = new_block_buffer_size(device_, kHistBytes, n);
     for (i32 i = 0; i < n; ++i) {
       const Frame* f = frames[i].as_const_frame();
-      if (f->layout != FrameLayout::HWC || f->channels() != 3 || (proto::FrameType)f->type != proto::U8)
-        LOG(FATAL) << "Histogram expects HxWx3 uint8 frames, got " << f->height() << "x" << f->width() << "x"
-                   << f->channels();
+      if (f->layout != FrameLayout::HWC || f->channels() != 3 || (proto::FrameType)f->type != proto::U8) {
+        report_kernel_error("Histogram, row " + std::to_string(frames[i].index) + ": expects HxWx3 uint8 frames, got " +
+                            std::to_string(f->height()) + "x" + std::to_string(f->width()) + "x" +
+                            std::to_string(f->channels()) + " type " + std::to_string((int)(proto::FrameType)f->type) +
+                            (f->layout == FrameLayout::HWC ? "" : " (an NV12 frame element)"));
+        output_columns[0].push_back(Element());
+        delete_buffer(device_, block);  // the refused row's reference
+        continue;
+      }
       i32* out = reinterpret_cast<i32*>(block + (size_t)i * kHistBytes);
       // four sub-histograms per channel break the store-to-load chain on runs of equal values
       i32 part[4][3][16];

@@ -71,25 +71,40 @@ class HistogramKernelGPU : public BatchedKernel {
     if (n == 0) return;
     CU_CHECK(cudaSetDevice(device_.id));
     constexpr size_t kHistBytes = 3 * 16 * sizeof(i32);
-    u8* block = new_block_buffer_size(device_, kHistBytes, n);  // one block for the batch
+    u8* block = new_block_buffer_size(device_, kHistBytes, n);  // one block for the batch, one reference per row
+    std::vector<bool> refused(n, false);
     for_each_run(frames, [&](size_t i0, size_t i1, const Frame* f0) {
-      require_rgb8(f0, "Histogram");
-      std::vector<const u8*> ptrs;
-      for (size_t i = i0; i < i1; ++i) ptrs.push_back(frames[i].as_const_frame()->data);
-      if (is_nv12(f0)) {
-        // decoder-native surface: colour conversion happens in registers, RGB24 never exists
-        const int w = pic_width(f0), h = pic_height(f0);
-        std::vector<const u8*> chroma;
-        for (const u8* p : ptrs) chroma.push_back(p + (size_t)w * h);
-        SCN_CHECK(scn_nv12_hist_resize(ptrs.data(), chroma.data(), (size_t)w, (int)ptrs.size(), w, h,
-                                       (int32_t*)(block + i0 * kHistBytes), nullptr, 0, 0, nullptr,
-                                       device_stream(device_)));
-        return;
+      std::string why = rgb8_problem(f0);
+      int rc = 0;
+      if (why.empty()) {
+        std::vector<const u8*> ptrs;
+        for (size_t i = i0; i < i1; ++i) ptrs.push_back(frames[i].as_const_frame()->data);
+        if (is_nv12(f0)) {
+          // decoder-native surface: colour conversion happens in registers, RGB24 never exists
+          const int w = pic_width(f0), h = pic_height(f0);
+          std::vector<const u8*> chroma;
+          for (const u8* p : ptrs) chroma.push_back(p + (size_t)w * h);
+          rc = scn_nv12_hist_resize(ptrs.data(), chroma.data(), (size_t)w, (int)ptrs.size(), w, h,
+                                    (int32_t*)(block + i0 * kHistBytes), nullptr, 0, 0, nullptr, device_stream(device_));
+        } else {
+          rc = scn_hist16_u8c3(ptrs.data(), (int)ptrs.size(), f0->width(), f0->height(),
+                               (int32_t*)(block + i0 * kHistBytes), device_stream(device_));
+        }
+        if (rc == 0) return;
+        why = std::string(is_nv12(f0) ? "scn_nv12_hist_resize" : "scn_hist16_u8c3") + " failed with code " +
+              std::to_string(rc);
       }
-      SCN_CHECK(scn_hist16_u8c3(ptrs.data(), (int)ptrs.size(), f0->width(), f0->height(),
-                                (int32_t*)(block + i0 * kHistBytes), device_stream(device_)));
+      report_kernel_error("Histogram, row " + std::to_string(frames[i0].index) + ": " + why);
+      for (size_t i = i0; i < i1; ++i) refused[i] = true;
     });
-    for (i32 i = 0; i < n; ++i) insert_element(output_columns[0], block + (size_t)i * kHistBytes, kHistBytes);
+    for (i32 i = 0; i < n; ++i) {
+      if (!refused[i]) {
+        insert_element(output_columns[0], block + (size_t)i * kHistBytes, kHistBytes);
+      } else {
+        output_columns[0].push_back(Element());
+        delete_buffer(device_, block);  // the refused row's reference
+      }
+    }
   }
 
  private:
@@ -294,18 +309,32 @@ class BlurKernelGPU : public BatchedKernel {
     if (frames.empty()) return;
     CU_CHECK(cudaSetDevice(device_.id));
     for_each_run(frames, [&](size_t i0, size_t i1, const Frame* f0) {
-      require_rgb8(f0, "Blur");
       const i32 n = (i32)(i1 - i0);
-      std::vector<Frame*> outs = new_frames(device_, f0->as_frame_info(), n);
-      std::vector<const u8*> src;
-      std::vector<u8*> dst;
-      for (i32 i = 0; i < n; ++i) {
-        src.push_back(frames[i0 + i].as_const_frame()->data);
-        dst.push_back(outs[i]->data);
+      // Blur takes dense RGB24 only (it declares no NV12 input layout)
+      std::string why = is_nv12(f0) ? "expects HxWx3 uint8 frames, got an NV12 frame element" : rgb8_problem(f0);
+      if (why.empty()) {
+        std::vector<Frame*> outs = new_frames(device_, f0->as_frame_info(), n);
+        std::vector<const u8*> src;
+        std::vector<u8*> dst;
+        for (i32 i = 0; i < n; ++i) {
+          src.push_back(frames[i0 + i].as_const_frame()->data);
+          dst.push_back(outs[i]->data);
+        }
+        const int rc = scn_box_blur_u8c3(src.data(), n, f0->width(), f0->height(), kernel_size_, dst.data(),
+                                         device_stream(device_));
+        if (rc == 0) {
+          for (i32 i = 0; i < n; ++i) insert_frame(output_columns[0], outs[i]);
+          return;
+        }
+        for (Frame* f : outs) {
+          delete_buffer(device_, f->data);
+          delete f;
+        }
+        why = "scn_box_blur_u8c3 failed with code " + std::to_string(rc) + " on " + std::to_string(n) + " " +
+              std::to_string(f0->height()) + "x" + std::to_string(f0->width()) + " frames";
       }
-      SCN_CHECK(scn_box_blur_u8c3(src.data(), n, f0->width(), f0->height(), kernel_size_, dst.data(),
-                                  device_stream(device_)));
-      for (i32 i = 0; i < n; ++i) insert_frame(output_columns[0], outs[i]);
+      report_kernel_error("Blur, row " + std::to_string(frames[i0].index) + ": " + why);
+      for (i32 i = 0; i < n; ++i) output_columns[0].push_back(Element());
     });
   }
 

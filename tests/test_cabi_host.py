@@ -135,6 +135,37 @@ def test_bad_arguments_are_rejected_without_a_gpu():
     assert l.scn_nv12_to_rgb24(None, None, 8, 1, 7, 8, None, 24, None) == -1  # odd width
 
 
+BLUR_REFUSALS = [  # (n, width, height, kernel_size, expected return code)
+    (-1, 16, 16, 3, -1), (1, 16, 16, 0, -1), (1, 16, 16, 32, -1), (1, 0, 16, 3, -1), (1, 16, 0, 3, -1),
+    (1, (1 << 29) + 1, 1, 3, -1), (1, 2**31 - 1, 1, 1, -1), (0, 2**31 - 1, 1, 1, -1),
+    (1, 1, 65535 * 32 + 1, 3, -2), (2, 16, 2**31 - 1, 3, -2), (1, 1 << 29, 2**31 - 1, 31, -2),
+]
+
+
+def test_blur_refusals_launch_nothing_and_write_nothing():
+    """scn_box_blur_u8c3 refuses before any launch: n < 0, kernel sizes 0 and 32, null pointer lists, a width past
+    2^29 (row offsets are int arithmetic), and, with SCN_E_UNSUPPORTED, frames taller than 2,097,120 rows (the
+    generic kernel's grid), INT_MAX included, whose rounding up to a strip would overflow int.  The pointers name
+    host buffers: a refusal never dereferences them."""
+    l = cabi.lib()
+    src, dst = np.arange(64, dtype=np.uint8), np.full(64, 0x5A, np.uint8)
+    before = l.scn_launch_count()
+    for (n, w, h, k, rc) in BLUR_REFUSALS:
+        ps, keep_s = cabi.ptr_array([src.ctypes.data] * max(n, 1))
+        pd, keep_d = cabi.ptr_array([dst.ctypes.data] * max(n, 1))
+        assert l.scn_box_blur_u8c3(ps, n, w, h, k, pd, None) == rc, (n, w, h, k)
+        assert l.scn_box_blur_u8c3_strided(src.ctypes.data, 0, n, w, h, k, dst.ctypes.data, None) == rc, (n, w, h, k)
+    for n in (1, 3):
+        ps, keep_s = cabi.ptr_array([src.ctypes.data] * n)
+        assert l.scn_box_blur_u8c3(None, n, 16, 16, 3, ps, None) == -1
+        assert l.scn_box_blur_u8c3(ps, n, 16, 16, 3, None, None) == -1
+        assert l.scn_box_blur_u8c3_strided(None, 48, n, 16, 16, 3, dst.ctypes.data, None) == -1
+        assert l.scn_box_blur_u8c3_strided(src.ctypes.data, 48, n, 16, 16, 3, None, None) == -1
+    assert l.scn_box_blur_u8c3(None, 0, 16, 16, 3, None, None) == 0  # n == 0 is a no-op
+    assert l.scn_launch_count() == before
+    assert (dst == 0x5A).all() and (src == np.arange(64)).all()
+
+
 def test_nv12_stream_unit_division_by_multiply_shift_is_exact():
     """nv12_stream_kernel splits a unit index u (16 pixels x 2 rows) into row pair and column with
     (u * (floor(2^32 / upr) + 1)) >> 32, upr = width / 16 (nvs::launch, nvs::Params::upr_recip).  Exhaustive over every

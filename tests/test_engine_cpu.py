@@ -394,6 +394,34 @@ def test_config0_as_stated_h264_clip_histogram_on_a_cpu_instance(tmp_path):
     e1.close()
 
 
+def test_cpu_histogram_fails_the_run_on_gray_and_float_frames_and_the_engine_goes_on():
+    """The stdlib Histogram on a CPU instance refuses frames that are not HxWx3 uint8 by failing the run with the
+    op, the row and the reason; the process lives and the same engine then runs a valid Histogram."""
+    E.load_stdlib()
+    eng = E.Engine(gpus=[], cpu_instances=1)
+    try:
+        def run(frames):
+            g = E.Graph()
+            src = g.add_source(True)
+            sink = g.add_sink((g.add_op("Histogram", [(src, "frame")], device=0), "histogram"))
+            j = E.Job()
+            j.bind_source(src, eng.add_raw_frames(frames))
+            eng.run(g, [j], 4, 8)
+            return j, sink
+        gray = np.random.default_rng(3).integers(0, 256, (3, 6, 10, 1), dtype=np.uint8)
+        with pytest.raises(E.EngineError, match=r"Histogram, row 0: expects HxWx3 uint8 frames, got 6x10x1"):
+            run(gray)
+        with pytest.raises(E.EngineError, match=r"Histogram, row 0: expects HxWx3 uint8 frames, got 5x7x3 type 1"):
+            run(np.zeros((2, 5, 7, 3), np.float32))
+        rgb = np.stack([synth.rand_frame(60 + i, 9, 11) for i in range(5)])
+        j, sink = run(rgb)
+        hist = j.output_array(sink, 192, np.int32).reshape(5, 3, 16)
+        for i in range(5):
+            assert (hist[i] == oracle.hist16(rgb[i])).all(), i
+    finally:
+        eng.close()
+
+
 @pytest.mark.parametrize("mode,gop", [("pcm", 4), ("skip", 5), ("bidir", 6)])
 def test_cpu_instance_decodes_sampled_rows_of_every_stream_kind(tmp_path, mode, gop):
     """Gather over keyframe intervals on the software path: only the intervals that hold wanted rows are fed, B

@@ -28,7 +28,13 @@ from oracle.recorded import Answers  # noqa: E402
 
 REF_SO = os.path.join(ROOT, "oracle", "_ref", "libref_test_ops.so")
 TEST_OPS_SO = os.path.join(ROOT, "build", "tests", "libtest_plugin_ops.so")
-BLUR_CASES = [(3, 37, 53, 3), (4, 40, 31, 2), (5, 64, 48, 2), (8, 33, 47, 1), (15, 40, 56, 1)]
+# (k, h, w, frames): every kernel size on a frame a few pixels larger than the window, and frames whose interior is
+# empty (a side shorter than the window, one row, one column) or a single pixel (both sides equal to the window)
+BLUR_CASES = ([(3, 37, 53, 3), (4, 40, 31, 2), (5, 64, 48, 2), (8, 33, 47, 1), (15, 40, 56, 1)] +
+              [(k, k + 5, 2 * k + 3, 1) for k in range(1, 32)] +
+              [(k, k, k, 1) for k in (1, 2, 3, 4, 16, 30, 31)] +
+              [(k, k - 1, 40, 1) for k in (2, 3, 17, 31)] + [(k, 40, k - 1, 1) for k in (2, 4, 31)] +
+              [(k, 1, 37, 1) for k in (2, 3, 31)] + [(k, 37, 1, 1) for k in (2, 5, 31)])
 
 PRELUDE = r'''
 import hashlib, json, os, struct, sys
