@@ -23,15 +23,14 @@
 //   h264_scan_kernel       one CTA per frame: macroblock bit counts -> bit offsets after the slice header
 //   h264_count_epb_kernel  emulation-prevention bytes per 4 KiB chunk of each frame's payload
 //   h264_stuff_kernel      copies each chunk with its 0x03 bytes after the NAL prefix (SPS + PPS for an IDR)
-// The host reads back each frame's bit count and its emulation-prevention count, as the JPEG encoder does.
+// The last two are the output stage of bitstream.cuh with the escape rule EmulationPrevention, as in jpeg.cu.
 // Lane roles in h264_mb_kernel: lanes 0-15 are the 16 luma 4x4 blocks (raster order), lanes 16-19 the Cb and
 // 20-23 the Cr 4x4 blocks; lanes 24-31 only help load neighbours.
 #include <cuda_runtime.h>
 
-#include <cstring>
 #include <vector>
 
-#include "scn_common.cuh"
+#include "bitstream.cuh"
 
 namespace scn {
 namespace {
@@ -40,8 +39,7 @@ constexpr int kMaxSide = 4096;
 constexpr int kMaxMbs = 36864;  // MaxFS of level 5.1
 constexpr int kWarps = 16;      // macroblocks in flight per frame
 constexpr int kThreads = 128;   // h264_bits_kernel
-constexpr int kChunk = 4096;    // bytes of payload per CTA of the emulation-prevention passes
-constexpr int kMaxPrefix = 96;
+constexpr int kMaxNalPrefix = 96;  // at most this many bytes (SPS, PPS, the slice's NAL header) precede a payload
 constexpr int kLevelMax = 2063;  // the largest |level| a level_prefix <= 15 codes at suffixLength 0
 constexpr uint32_t kFull = 0xFFFFFFFFu;
 
@@ -571,90 +569,39 @@ h264_scan_kernel(int i0, int nm, const __grid_constant__ SliceHeads heads, uint3
   if (threadIdx.x == 0) total[f] = (heads.len[blockIdx.x] + all + 1 + 7) / 8 * 8;
 }
 
-struct StreamSlots {
-  uint64_t stream_off[SCN_MAX_PTRS];  // byte offset of each frame's payload
-  uint64_t bytes[SCN_MAX_PTRS];       // bytes of each frame's payload (before emulation prevention)
-  uint64_t chunk_off[SCN_MAX_PTRS];   // index of each frame's first chunk count
-  uint64_t out_off[SCN_MAX_PTRS];     // byte offset of each frame's access unit in the output
-  uint8_t idr[SCN_MAX_PTRS];
-};
-
 // Emulation prevention (7.4.1): 0x03 goes before payload byte i when it is <= 3 and follows z >= 2 zero bytes with z
-// even (counting the payload's own zeros, not inserted bytes).  Returns the zero run before byte `at`.
-__device__ __forceinline__ int zeros_before(const uint8_t* p, uint64_t at) {
-  int z = 0;
-  while (at > 0 && p[at - 1] == 0) --at, ++z;
-  return z;
-}
-// number of 0x03 bytes the 16 bytes at p + at need (`valid` of them are payload)
-__device__ __forceinline__ int count_epb(const uint8_t* p, uint64_t at, const uint4& v, int valid) {
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-  int z = zeros_before(p, at), c = 0;
-  for (int k = 0; k < valid; ++k) {
-    const uint32_t b = (w[k >> 2] >> (8 * (k & 3))) & 0xFF;
-    c += b <= 3 && z >= 2 && !(z & 1);
-    z = b ? 0 : z + 1;
+// even (counting the payload's own zeros, not inserted bytes).
+struct EmulationPrevention {
+  static constexpr const char* count_name = "h264_count_epb_kernel";
+  static constexpr const char* copy_name = "h264_stuff_kernel";
+  static __device__ __forceinline__ int zeros_before(const uint8_t* p, uint64_t at) {
+    int z = 0;
+    while (at > 0 && p[at - 1] == 0) --at, ++z;
+    return z;
   }
-  return c;
-}
-
-__global__ void __launch_bounds__(256)
-h264_count_epb_kernel(int i0, const __grid_constant__ StreamSlots s, const uint8_t* streams, uint32_t* chunk_epb,
-                      unsigned long long* epb) {
-  const int j = blockIdx.y;
-  const uint64_t bytes = s.bytes[j];
-  const uint64_t at = (uint64_t)blockIdx.x * kChunk;
-  if (at >= bytes) return;
-  const uint8_t* p = streams + s.stream_off[j];
-  const uint64_t i = at + threadIdx.x * 16;
-  int c = 0;
-  if (i < bytes) c = count_epb(p, i, *reinterpret_cast<const uint4*>(p + i), (int)min(bytes - i, (uint64_t)16));
-  unsigned long long total;
-  block_exclusive_scan<unsigned long long>((unsigned long long)c, &total);
-  if (threadIdx.x == 0) {
-    chunk_epb[s.chunk_off[j] + blockIdx.x] = (uint32_t)total;
-    atomicAdd(epb + i0 + j, total);
+  static __device__ __forceinline__ int count(const uint8_t* p, uint64_t at, const uint4& v, int valid) {
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    int z = zeros_before(p, at), c = 0;
+    for (int k = 0; k < valid; ++k) {
+      const uint32_t b = (w[k >> 2] >> (8 * (k & 3))) & 0xFF;
+      c += b <= 3 && z >= 2 && !(z & 1);
+      z = b ? 0 : z + 1;
+    }
+    return c;
   }
-}
-
-struct Prefixes {
-  uint8_t b[2][kMaxPrefix];  // [idr]: start code and NAL header of the slice, after SPS + PPS for an IDR
-  int len[2];
+  static __device__ __forceinline__ uint8_t* copy(const uint8_t* p, uint64_t at, const uint4& v, int valid,
+                                                  uint8_t* o) {
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    int z = zeros_before(p, at);
+    for (int k = 0; k < valid; ++k) {
+      const uint8_t b = (uint8_t)(w[k >> 2] >> (8 * (k & 3)));
+      if (b <= 3 && z >= 2 && !(z & 1)) *o++ = 3;
+      *o++ = b;
+      z = b ? 0 : z + 1;
+    }
+    return o;
+  }
 };
-
-__global__ void __launch_bounds__(256)
-h264_stuff_kernel(const __grid_constant__ StreamSlots s, const __grid_constant__ Prefixes pre, const uint8_t* streams,
-                  const uint32_t* chunk_epb, uint8_t* out) {
-  const int j = blockIdx.y;
-  const uint64_t bytes = s.bytes[j];
-  const uint64_t at = (uint64_t)blockIdx.x * kChunk;
-  if (at >= bytes) return;
-  const int kind = s.idr[j];
-  uint8_t* au = out + s.out_off[j];
-  if (blockIdx.x == 0)
-    for (int k = threadIdx.x; k < pre.len[kind]; k += blockDim.x) au[k] = pre.b[kind][k];
-  unsigned long long before = 0;
-  for (uint32_t c = threadIdx.x; c < blockIdx.x; c += blockDim.x) before += chunk_epb[s.chunk_off[j] + c];
-  unsigned long long chunk_before;
-  block_exclusive_scan<unsigned long long>(before, &chunk_before);
-  const uint8_t* p = streams + s.stream_off[j];
-  const uint64_t i = at + threadIdx.x * 16;
-  uint4 v = make_uint4(0, 0, 0, 0);
-  const int valid = i < bytes ? (int)min(bytes - i, (uint64_t)16) : 0;
-  if (valid) v = *reinterpret_cast<const uint4*>(p + i);
-  unsigned long long total;
-  const unsigned long long mine =
-      block_exclusive_scan<unsigned long long>((unsigned long long)(valid ? count_epb(p, i, v, valid) : 0), &total);
-  uint8_t* o = au + pre.len[kind] + i + chunk_before + mine;
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-  int z = valid ? zeros_before(p, i) : 0;
-  for (int k = 0; k < valid; ++k) {
-    const uint8_t b = (uint8_t)(w[k >> 2] >> (8 * (k & 3)));
-    if (b <= 3 && z >= 2 && !(z & 1)) *o++ = 3;
-    *o++ = b;
-    z = b ? 0 : z + 1;
-  }
-}
 
 // ---- host: parameter sets and slice headers ----
 struct Bits {
@@ -794,7 +741,7 @@ extern "C" size_t scn_h264_encode_bound(int width, int height) {
   const Geom g = make_geom(width, height);
   if (g.mbs() > kMaxMbs) return 0;
   const size_t payload = ((size_t)g.mbs() * kWorstMbBits + 64) / 8 + 1;
-  return (size_t)kMaxPrefix + payload + payload / 2 + 1;  // at most one 0x03 per two payload bytes
+  return (size_t)kMaxNalPrefix + payload + payload / 2 + 1;  // at most one 0x03 per two payload bytes
 }
 
 extern "C" int scn_h264_encode_u8(const uint8_t* const* host_src_ptrs, int n, int width, int height, int qp,
@@ -822,18 +769,13 @@ extern "C" int scn_h264_encode_u8(const uint8_t* const* host_src_ptrs, int n, in
     slice_header(pos, keyframe_distance, &head_bits[i], &head_len[i], &key);
     idr[i] = key;
   }
-  Prefixes pre = {};
-  {
-    std::vector<uint8_t> key;
-    append_nal(key, 3, 7, sps(g));
-    append_nal(key, 3, 8, pps(qp));
-    key.insert(key.end(), {0, 0, 0, 1, 3 << 5 | 5});
-    const std::vector<uint8_t> other = {0, 0, 0, 1, 2 << 5 | 1};
-    std::memcpy(pre.b[1], key.data(), key.size());
-    pre.len[1] = (int)key.size();
-    std::memcpy(pre.b[0], other.data(), other.size());
-    pre.len[0] = (int)other.size();
-  }
+  // prefix 0 starts a non-IDR picture's access unit, prefix 1 (SPS, PPS, then the slice NAL) an IDR picture's
+  std::vector<uint8_t> key;
+  append_nal(key, 3, 7, sps(g));
+  append_nal(key, 3, 8, pps(qp));
+  key.insert(key.end(), {0, 0, 0, 1, 3 << 5 | 5});
+  Affixes ax;
+  if (!make_affixes(&ax, {0, 0, 0, 1, 2 << 5 | 1}, key, {})) return SCN_E_UNSUPPORTED;
   auto heads = [&](int i0, int cnt) {
     SliceHeads h = {};
     for (int j = 0; j < cnt; ++j) h.bits[j] = head_bits[i0 + j], h.len[j] = head_len[i0 + j];
@@ -844,94 +786,38 @@ extern "C" int scn_h264_encode_u8(const uint8_t* const* host_src_ptrs, int n, in
   MbRec* recs = s.get<MbRec>((size_t)n * nm, pool);
   uint8_t* recon = s.get<uint8_t>((size_t)(n < SCN_MAX_PTRS ? n : SCN_MAX_PTRS) * g.rec_bytes(), pool);
   uint32_t* mb_bit = s.get<uint32_t>((size_t)n * nm, pool);
-  uint64_t* totals = s.get<uint64_t>((size_t)n * 2, pool);  // payload bits per frame, then 0x03 bytes per frame
-  if (!recs || !recon || !mb_bit || !totals) return (int)cudaErrorMemoryAllocation;
-  unsigned long long* epbs = reinterpret_cast<unsigned long long*>(totals + n);
+  uint64_t* bits = s.get<uint64_t>((size_t)n, pool);
+  if (!recs || !recon || !mb_bit || !bits) return (int)cudaErrorMemoryAllocation;
   const int qpc = chroma_qp(qp);
   const unsigned mb_blocks = (unsigned)((nm + kThreads - 1) / kThreads);
 
-  // 1. the wavefront, macroblock bit counts, per-frame scans into bit offsets
-  int rc = for_each_chunk(n, [&](int i0, int cnt) {
-    const PtrBatch src = gather<PtrBatch>(host_src_ptrs, i0, cnt);
-    int e = launch_kernel("h264_mb_kernel", st, [&] {
-      h264_mb_kernel<<<cnt, kWarps * 32, 0, st>>>(src, i0, g, qp, qpc, recs, recon);
+  // the wavefront, macroblock bit counts, per-frame scans into bit offsets
+  auto measure = [&] {
+    return for_each_chunk(n, [&](int i0, int cnt) {
+      const PtrBatch src = gather<PtrBatch>(host_src_ptrs, i0, cnt);
+      int e = launch_kernel("h264_mb_kernel", st, [&] {
+        h264_mb_kernel<<<cnt, kWarps * 32, 0, st>>>(src, i0, g, qp, qpc, recs, recon);
+      });
+      if (e) return e;
+      const SliceHeads h = heads(i0, cnt);
+      e = launch_kernel("h264_bits_kernel<count>", st, [&] {
+        h264_bits_kernel<false><<<dim3(mb_blocks, (unsigned)cnt), kThreads, 0, st>>>(i0, g, recs, mb_bit, h, EmitIn{});
+      });
+      if (e) return e;
+      return launch_kernel("h264_scan_kernel", st, [&] {
+        h264_scan_kernel<<<cnt, 1024, 0, st>>>(i0, nm, h, mb_bit, bits);
+      });
     });
-    if (e) return e;
-    const SliceHeads h = heads(i0, cnt);
-    e = launch_kernel("h264_bits_kernel<count>", st, [&] {
-      h264_bits_kernel<false><<<dim3(mb_blocks, (unsigned)cnt), kThreads, 0, st>>>(i0, g, recs, mb_bit, h, EmitIn{});
-    });
-    if (e) return e;
-    return launch_kernel("h264_scan_kernel", st, [&] {
-      h264_scan_kernel<<<cnt, 1024, 0, st>>>(i0, nm, h, mb_bit, totals);
-    });
-  });
-  if (rc) return rc;
-  std::vector<uint64_t> bits((size_t)n);
-  if ((rc = (int)cudaMemcpyAsync(bits.data(), totals, (size_t)n * 8, cudaMemcpyDeviceToHost, st))) return rc;
-  if ((rc = (int)cudaStreamSynchronize(st))) return rc;
-
-  // 2. each frame's payload into scratch sized from the counts, and its emulation-prevention count
-  std::vector<uint64_t> stream_off((size_t)n), bytes((size_t)n), chunk_off((size_t)n);
-  uint64_t stream_total = 0, chunks = 0, max_chunks = 0;
-  for (int i = 0; i < n; ++i) {
-    bytes[i] = bits[i] / 8;
-    stream_off[i] = stream_total;
-    stream_total += (bytes[i] + 15) / 16 * 16;
-    chunk_off[i] = chunks;
-    const uint64_t c = (bytes[i] + kChunk - 1) / kChunk;
-    chunks += c;
-    max_chunks = c > max_chunks ? c : max_chunks;
-  }
-  uint8_t* streams = s.get<uint8_t>(stream_total, pool);
-  uint32_t* chunk_epb = s.get<uint32_t>(chunks, pool);
-  if (!streams || !chunk_epb) return (int)cudaErrorMemoryAllocation;
-  if ((rc = (int)cudaMemsetAsync(streams, 0, stream_total, st))) return rc;
-  if ((rc = (int)cudaMemsetAsync(epbs, 0, (size_t)n * 8, st))) return rc;
-  auto slots = [&](int i0, int cnt, const std::vector<uint64_t>& out_off) {
-    StreamSlots sl = {};
-    for (int j = 0; j < cnt; ++j) {
-      sl.stream_off[j] = stream_off[i0 + j];
-      sl.bytes[j] = bytes[i0 + j];
-      sl.chunk_off[j] = chunk_off[i0 + j];
-      sl.out_off[j] = out_off.empty() ? 0 : out_off[i0 + j];
-      sl.idr[j] = idr[i0 + j];
-    }
-    return sl;
   };
-  rc = for_each_chunk(n, [&](int i0, int cnt) {
+  // each macroblock's bits at its offset in its frame's payload
+  auto emit = [&](int i0, int cnt, uint8_t* streams, const uint64_t* stream_off) {
     EmitIn ei = {streams, {}};
-    for (int j = 0; j < cnt; ++j) ei.stream_off[j] = stream_off[i0 + j];
+    for (int j = 0; j < cnt; ++j) ei.stream_off[j] = stream_off[j];
     const SliceHeads h = heads(i0, cnt);
-    const int e = launch_kernel("h264_bits_kernel<emit>", st, [&] {
+    return launch_kernel("h264_bits_kernel<emit>", st, [&] {
       h264_bits_kernel<true><<<dim3(mb_blocks, (unsigned)cnt), kThreads, 0, st>>>(i0, g, recs, mb_bit, h, ei);
     });
-    if (e) return e;
-    const StreamSlots sl = slots(i0, cnt, {});
-    return launch_kernel("h264_count_epb_kernel", st, [&] {
-      h264_count_epb_kernel<<<dim3((unsigned)max_chunks, (unsigned)cnt), 256, 0, st>>>(i0, sl, streams, chunk_epb,
-                                                                                      epbs);
-    });
-  });
-  if (rc) return rc;
-  std::vector<uint64_t> epb((size_t)n);
-  if ((rc = (int)cudaMemcpyAsync(epb.data(), epbs, (size_t)n * 8, cudaMemcpyDeviceToHost, st))) return rc;
-  if ((rc = (int)cudaStreamSynchronize(st))) return rc;
-
-  // 3. the access units, back to back in the caller's buffer
-  std::vector<uint64_t> out_off((size_t)n);
-  size_t out_total = 0;
-  for (int i = 0; i < n; ++i) {
-    host_sizes[i] = (size_t)pre.len[idr[i]] + bytes[i] + epb[i];
-    out_off[i] = out_total;
-    out_total += host_sizes[i];
-  }
-  uint8_t* out = static_cast<uint8_t*>(alloc_out(alloc_ctx, out_total));
-  if (!out) return SCN_E_ALLOC;
-  return for_each_chunk(n, [&](int i0, int cnt) {
-    const StreamSlots sl = slots(i0, cnt, out_off);
-    return launch_kernel("h264_stuff_kernel", st, [&] {
-      h264_stuff_kernel<<<dim3((unsigned)max_chunks, (unsigned)cnt), 256, 0, st>>>(sl, pre, streams, chunk_epb, out);
-    });
-  });
+  };
+  return run_output_stage<EmulationPrevention>(n, st, pool, s, bits, idr.data(), ax, measure, emit, alloc_out,
+                                               alloc_ctx, host_sizes);
 }

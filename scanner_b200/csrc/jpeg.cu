@@ -19,22 +19,19 @@
 //                              an MCU shares with its neighbours with atomicOr)
 //   jpeg_count_ff_kernel       0xFF bytes per 4 KiB chunk of each frame's bit stream
 //   jpeg_stuff_kernel          copies each chunk with a 0x00 after every 0xFF, and places the header and EOI
-// The host reads back each frame's bit count (to size the bit streams) and its 0xFF count (to size the output):
-// two small copies, each behind a stream synchronisation.
+// The last two are the output stage of bitstream.cuh with the escape rule FfStuffing; the stage also reads back
+// each frame's bit count (to size the bit streams) and its 0xFF count (to size the output).
 #include <cuda_runtime.h>
 
-#include <cstring>
 #include <vector>
 
-#include "scn_common.cuh"
+#include "bitstream.cuh"
 
 namespace scn {
 namespace {
 
 constexpr int kMaxDim = 65500;  // libjpeg's JPEG_MAX_DIMENSION
 constexpr int kThreads = 128;   // MCU kernels
-constexpr int kChunk = 4096;    // bytes of bit stream per CTA of the 0xFF passes (256 threads x 16)
-constexpr int kMaxHeader = 640;
 
 // ---- tables (Annex K) ----
 constexpr uint8_t kLumaQ[64] = {16, 11, 10, 16, 24,  40,  51,  61,  12, 12, 14, 19, 26,  58,  60,  55,
@@ -124,13 +121,9 @@ Tables make_tables(int quality) {
   return t;
 }
 
-struct Header {
-  uint8_t b[kMaxHeader];
-  int len;
-};
-
-// SOI, APP0 (JFIF 1.01, no units, density 1 x 1), DQT per table, SOF0, DHT per table (DC0 AC0 DC1 AC1), SOS.
-Header make_header(int w, int h, int channels, int quality) {
+// SOI, APP0 (JFIF 1.01, no units, density 1 x 1), DQT per table, SOF0, DHT per table (DC0 AC0 DC1 AC1), SOS:
+// 623 bytes in colour, within the output stage's kMaxPrefix.
+std::vector<uint8_t> make_header(int w, int h, int channels, int quality) {
   std::vector<uint8_t> o = {0xFF, 0xD8};
   auto marker = [&](uint8_t m, const std::vector<uint8_t>& p) {
     const size_t len = p.size() + 2;
@@ -164,10 +157,7 @@ Header make_header(int w, int h, int channels, int quality) {
     marker(0xDA, {3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0});
   else
     marker(0xDA, {1, 1, 0x00, 0, 63, 0});
-  Header hd;
-  hd.len = (int)o.size();
-  std::memcpy(hd.b, o.data(), o.size());
-  return hd;
+  return o;
 }
 
 // ---- geometry ----
@@ -460,73 +450,27 @@ jpeg_scan_kernel(int i0, uint32_t nm, int bpm, Tables tables, const int16_t* dcs
   if (threadIdx.x == 0) total[f] = all;
 }
 
-struct StreamSlots {
-  uint64_t stream_off[SCN_MAX_PTRS];  // byte offset of each frame's bit stream
-  uint64_t bytes[SCN_MAX_PTRS];       // bytes of each frame's bit stream (unstuffed)
-  uint64_t chunk_off[SCN_MAX_PTRS];   // index of each frame's first chunk count
-  uint64_t out_off[SCN_MAX_PTRS];     // byte offset of each frame's file in the output
-};
-
-// 0xFF bytes among the 16 bytes at p, of which the first `valid` count
-__device__ __forceinline__ int count_ff(const uint4& v, int64_t valid) {
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-  int c = 0;
+// B.1.1.5: a 0x00 after every 0xFF of the scan
+struct FfStuffing {
+  static constexpr const char* count_name = "jpeg_count_ff_kernel";
+  static constexpr const char* copy_name = "jpeg_stuff_kernel";
+  static __device__ __forceinline__ int count(const uint8_t*, uint64_t, const uint4& v, int valid) {
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    int c = 0;
 #pragma unroll
-  for (int k = 0; k < 16; ++k) c += (k < valid) && ((w[k >> 2] >> (8 * (k & 3))) & 0xFF) == 0xFF;
-  return c;
-}
-
-__global__ void __launch_bounds__(256)
-jpeg_count_ff_kernel(int i0, StreamSlots s, const uint8_t* streams, uint32_t* chunk_ff, unsigned long long* ff) {
-  const int j = blockIdx.y;
-  const uint64_t bytes = s.bytes[j];
-  const uint64_t at = (uint64_t)blockIdx.x * kChunk;
-  if (at >= bytes) return;
-  const uint64_t i = at + threadIdx.x * 16;
-  int c = 0;
-  if (i < bytes) c = count_ff(*reinterpret_cast<const uint4*>(streams + s.stream_off[j] + i), (int64_t)(bytes - i));
-  unsigned long long total;
-  block_exclusive_scan<unsigned long long>((unsigned long long)c, &total);
-  if (threadIdx.x == 0) {
-    chunk_ff[s.chunk_off[j] + blockIdx.x] = (uint32_t)total;
-    atomicAdd(ff + i0 + j, total);
+    for (int k = 0; k < 16; ++k) c += (k < valid) && ((w[k >> 2] >> (8 * (k & 3))) & 0xFF) == 0xFF;
+    return c;
   }
-}
-
-__global__ void __launch_bounds__(256)
-jpeg_stuff_kernel(const __grid_constant__ StreamSlots s, const __grid_constant__ Header hd, const uint8_t* streams,
-                  const uint32_t* chunk_ff, uint8_t* out) {
-  const int j = blockIdx.y;
-  const uint64_t bytes = s.bytes[j];
-  const uint64_t at = (uint64_t)blockIdx.x * kChunk;
-  if (at >= bytes) return;
-  uint8_t* file = out + s.out_off[j];
-  if (blockIdx.x == 0)
-    for (int k = threadIdx.x; k < hd.len; k += blockDim.x) file[k] = hd.b[k];
-  // 0xFF bytes of the chunks before this one
-  unsigned long long before = 0;
-  for (uint32_t c = threadIdx.x; c < blockIdx.x; c += blockDim.x) before += chunk_ff[s.chunk_off[j] + c];
-  unsigned long long chunk_before;
-  block_exclusive_scan<unsigned long long>(before, &chunk_before);
-  const uint64_t i = at + threadIdx.x * 16;
-  uint4 v = make_uint4(0, 0, 0, 0);
-  const int64_t valid = i < bytes ? (int64_t)(bytes - i < 16 ? bytes - i : 16) : 0;
-  if (valid) v = *reinterpret_cast<const uint4*>(streams + s.stream_off[j] + i);
-  unsigned long long total;
-  const unsigned long long mine =
-      block_exclusive_scan<unsigned long long>((unsigned long long)count_ff(v, valid), &total);
-  uint8_t* o = file + hd.len + i + chunk_before + mine;
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-  for (int k = 0; k < valid; ++k) {
-    const uint8_t b = (uint8_t)(w[k >> 2] >> (8 * (k & 3)));
-    *o++ = b;
-    if (b == 0xFF) *o++ = 0;
+  static __device__ __forceinline__ uint8_t* copy(const uint8_t*, uint64_t, const uint4& v, int valid, uint8_t* o) {
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    for (int k = 0; k < valid; ++k) {
+      const uint8_t b = (uint8_t)(w[k >> 2] >> (8 * (k & 3)));
+      *o++ = b;
+      if (b == 0xFF) *o++ = 0;
+    }
+    return o;
   }
-  if (valid && i + valid == bytes) {
-    o[0] = 0xFF;
-    o[1] = 0xD9;
-  }
-}
+};
 
 size_t worst_bits_per_block() { return 11 + 11 + 63 * (16 + 10); }  // DC code + value, 63 AC codes + values
 
@@ -539,7 +483,7 @@ extern "C" size_t scn_jpeg_encode_bound(int width, int height, int channels) {
   const Geom g = make_geom(width, height, channels);
   const size_t blocks = (size_t)g.mcus() * g.bpm;
   const size_t bytes = (blocks * worst_bits_per_block() + 7) / 8;
-  return (size_t)make_header(width, height, channels, 95).len + 2 * bytes + 2;
+  return make_header(width, height, channels, 95).size() + 2 * bytes + 2;
 }
 
 extern "C" int scn_jpeg_encode_u8(const uint8_t* const* host_src_ptrs, int n, int width, int height, int channels,
@@ -557,101 +501,48 @@ extern "C" int scn_jpeg_encode_u8(const uint8_t* const* host_src_ptrs, int n, in
   const Geom g = make_geom(width, height, channels);
   const uint32_t nm = g.mcus();
   const Tables tables = make_tables(quality);
-  const Header hd = make_header(width, height, channels, quality);
+  Affixes ax;
+  if (!make_affixes(&ax, make_header(width, height, channels, quality), {}, {0xFF, 0xD9})) return SCN_E_UNSUPPORTED;
 
   Scratch s{st, {}};
   int16_t* dcs = s.get<int16_t>((size_t)n * nm * g.bpm, pool);
   uint32_t* acbits = s.get<uint32_t>((size_t)n * nm, pool);
   uint64_t* mcu_bit = s.get<uint64_t>((size_t)n * nm, pool);
-  uint64_t* totals = s.get<uint64_t>((size_t)n * 2, pool);  // bits per frame, then 0xFF bytes per frame
-  if (!dcs || !acbits || !mcu_bit || !totals) return (int)cudaErrorMemoryAllocation;
-  unsigned long long* ffs = reinterpret_cast<unsigned long long*>(totals + n);
+  uint64_t* bits = s.get<uint64_t>((size_t)n, pool);
+  if (!dcs || !acbits || !mcu_bit || !bits) return (int)cudaErrorMemoryAllocation;
   const dim3 mcu_grid((nm + kThreads - 1) / kThreads);
 
-  // 1. measure: DCs and AC bit counts, then per-frame scans into bit offsets
-  int rc = for_each_chunk(n, [&](int i0, int cnt) {
-    const PtrBatch src = gather<PtrBatch>(host_src_ptrs, i0, cnt);
-    const MeasureOut mo = {dcs, acbits};
-    const dim3 grid(mcu_grid.x, (unsigned)cnt);
-    const int e = launch_kernel("jpeg_mcu_kernel<measure>", st, [&] {
-      if (channels == 3)
-        jpeg_mcu_kernel<3, false><<<grid, kThreads, 0, st>>>(src, i0, g, tables, mo, EmitIn{});
-      else
-        jpeg_mcu_kernel<1, false><<<grid, kThreads, 0, st>>>(src, i0, g, tables, mo, EmitIn{});
+  // DCs and AC bit counts, then per-frame scans into bit offsets
+  auto measure = [&] {
+    return for_each_chunk(n, [&](int i0, int cnt) {
+      const PtrBatch src = gather<PtrBatch>(host_src_ptrs, i0, cnt);
+      const MeasureOut mo = {dcs, acbits};
+      const dim3 grid(mcu_grid.x, (unsigned)cnt);
+      const int e = launch_kernel("jpeg_mcu_kernel<measure>", st, [&] {
+        if (channels == 3)
+          jpeg_mcu_kernel<3, false><<<grid, kThreads, 0, st>>>(src, i0, g, tables, mo, EmitIn{});
+        else
+          jpeg_mcu_kernel<1, false><<<grid, kThreads, 0, st>>>(src, i0, g, tables, mo, EmitIn{});
+      });
+      if (e) return e;
+      return launch_kernel("jpeg_scan_kernel", st, [&] {
+        jpeg_scan_kernel<<<cnt, 1024, 0, st>>>(i0, nm, g.bpm, tables, dcs, acbits, mcu_bit, bits);
+      });
     });
-    if (e) return e;
-    return launch_kernel("jpeg_scan_kernel", st, [&] {
-      jpeg_scan_kernel<<<cnt, 1024, 0, st>>>(i0, nm, g.bpm, tables, dcs, acbits, mcu_bit, totals);
-    });
-  });
-  if (rc) return rc;
-  std::vector<uint64_t> bits((size_t)n);
-  if ((rc = (int)cudaMemcpyAsync(bits.data(), totals, (size_t)n * 8, cudaMemcpyDeviceToHost, st))) return rc;
-  if ((rc = (int)cudaStreamSynchronize(st))) return rc;
-
-  // 2. emit each frame's bit stream into scratch sized from the counts, and count its 0xFF bytes
-  std::vector<uint64_t> stream_off((size_t)n), bytes((size_t)n), chunk_off((size_t)n);
-  uint64_t stream_total = 0, chunks = 0, max_chunks = 0;
-  for (int i = 0; i < n; ++i) {
-    bytes[i] = (bits[i] + 7) / 8;
-    stream_off[i] = stream_total;
-    stream_total += (bytes[i] + 15) / 16 * 16;
-    chunk_off[i] = chunks;
-    const uint64_t c = (bytes[i] + kChunk - 1) / kChunk;
-    chunks += c;
-    max_chunks = c > max_chunks ? c : max_chunks;
-  }
-  uint8_t* streams = s.get<uint8_t>(stream_total, pool);
-  uint32_t* chunk_ff = s.get<uint32_t>(chunks, pool);
-  if (!streams || !chunk_ff) return (int)cudaErrorMemoryAllocation;
-  if ((rc = (int)cudaMemsetAsync(streams, 0, stream_total, st))) return rc;
-  if ((rc = (int)cudaMemsetAsync(ffs, 0, (size_t)n * 8, st))) return rc;
-  auto slots = [&](int i0, int cnt, const std::vector<uint64_t>& out_off) {
-    StreamSlots sl = {};
-    for (int j = 0; j < cnt; ++j) {
-      sl.stream_off[j] = stream_off[i0 + j];
-      sl.bytes[j] = bytes[i0 + j];
-      sl.chunk_off[j] = chunk_off[i0 + j];
-      sl.out_off[j] = out_off.empty() ? 0 : out_off[i0 + j];
-    }
-    return sl;
   };
-  rc = for_each_chunk(n, [&](int i0, int cnt) {
+  // each MCU's bits at its offset in its frame's stream
+  auto emit = [&](int i0, int cnt, uint8_t* streams, const uint64_t* stream_off) {
     const PtrBatch src = gather<PtrBatch>(host_src_ptrs, i0, cnt);
-    EmitIn ei = {dcs, mcu_bit, totals, streams, {}};
-    for (int j = 0; j < cnt; ++j) ei.stream_off[j] = stream_off[i0 + j];
+    EmitIn ei = {dcs, mcu_bit, bits, streams, {}};
+    for (int j = 0; j < cnt; ++j) ei.stream_off[j] = stream_off[j];
     const dim3 grid(mcu_grid.x, (unsigned)cnt);
-    const int e = launch_kernel("jpeg_mcu_kernel<emit>", st, [&] {
+    return launch_kernel("jpeg_mcu_kernel<emit>", st, [&] {
       if (channels == 3)
         jpeg_mcu_kernel<3, true><<<grid, kThreads, 0, st>>>(src, i0, g, tables, MeasureOut{}, ei);
       else
         jpeg_mcu_kernel<1, true><<<grid, kThreads, 0, st>>>(src, i0, g, tables, MeasureOut{}, ei);
     });
-    if (e) return e;
-    const StreamSlots sl = slots(i0, cnt, {});
-    return launch_kernel("jpeg_count_ff_kernel", st, [&] {
-      jpeg_count_ff_kernel<<<dim3((unsigned)max_chunks, (unsigned)cnt), 256, 0, st>>>(i0, sl, streams, chunk_ff, ffs);
-    });
-  });
-  if (rc) return rc;
-  std::vector<uint64_t> ff((size_t)n);
-  if ((rc = (int)cudaMemcpyAsync(ff.data(), ffs, (size_t)n * 8, cudaMemcpyDeviceToHost, st))) return rc;
-  if ((rc = (int)cudaStreamSynchronize(st))) return rc;
-
-  // 3. the files, back to back in the caller's buffer
-  std::vector<uint64_t> out_off((size_t)n);
-  size_t out_total = 0;
-  for (int i = 0; i < n; ++i) {
-    host_sizes[i] = (size_t)hd.len + bytes[i] + ff[i] + 2;
-    out_off[i] = out_total;
-    out_total += host_sizes[i];
-  }
-  uint8_t* out = static_cast<uint8_t*>(alloc_out(alloc_ctx, out_total));
-  if (!out) return SCN_E_ALLOC;
-  return for_each_chunk(n, [&](int i0, int cnt) {
-    const StreamSlots sl = slots(i0, cnt, out_off);
-    return launch_kernel("jpeg_stuff_kernel", st, [&] {
-      jpeg_stuff_kernel<<<dim3((unsigned)max_chunks, (unsigned)cnt), 256, 0, st>>>(sl, hd, streams, chunk_ff, out);
-    });
-  });
+  };
+  return run_output_stage<FfStuffing>(n, st, pool, s, bits, nullptr, ax, measure, emit, alloc_out, alloc_ctx,
+                                      host_sizes);
 }

@@ -4,8 +4,6 @@
 #include <stdint.h>
 
 #include <atomic>
-#include <map>
-#include <mutex>
 #include <vector>
 
 #include "scn_kernels.h"
@@ -133,100 +131,5 @@ __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
   asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(sel));
   return r;
 }
-
-// ---- entropy coders' shared pieces (jpeg.cu, h264_enc.cu) ----
-
-// Appends bits MSB first to a frame's bit stream of big-endian 32-bit words.  The first and the last word a
-// writer touches may be shared with the neighbouring writers (MCUs, macroblocks) and are ORed in; the words between
-// are its own.
-struct BitWriter {
-  uint32_t* words;
-  uint64_t word;  // index of the word being filled
-  uint64_t acc;   // the low n bits are pending
-  int n;
-  bool first;
-  __device__ BitWriter(uint32_t* w, uint64_t bit) : words(w), word(bit >> 5), acc(0), n((int)(bit & 31)), first(true) {}
-  __device__ __forceinline__ void put(uint32_t bits, int len) {  // len <= 27
-    acc = (acc << len) | bits;
-    n += len;
-    if (n >= 32) {
-      n -= 32;
-      const uint32_t v = __byte_perm((uint32_t)(acc >> n), 0, 0x0123);
-      if (first) atomicOr(words + word, v);
-      else words[word] = v;
-      first = false;
-      ++word;
-    }
-  }
-  __device__ __forceinline__ void finish() {
-    if (n) atomicOr(words + word, __byte_perm((uint32_t)(acc << (32 - n)), 0, 0x0123));
-  }
-};
-
-// block-wide exclusive scan of one value per thread (blockDim.x a multiple of 32, at most 1024); returns the
-// exclusive prefix, *total the block's sum.  Every thread of the block calls it.
-template <class T>
-__device__ __forceinline__ T block_exclusive_scan(T v, T* total) {
-  __shared__ T warp_sums[32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  T x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const T y = __shfl_up_sync(0xFFFFFFFFu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp_sums[wid] = x;
-  __syncthreads();
-  if (wid == 0) {
-    T s = lane < nw ? warp_sums[lane] : 0;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const T y = __shfl_up_sync(0xFFFFFFFFu, s, o);
-      if (lane >= o) s += y;
-    }
-    warp_sums[lane] = s;  // inclusive
-  }
-  __syncthreads();
-  const T before = wid ? warp_sums[wid - 1] : 0;
-  *total = warp_sums[nw - 1];
-  __syncthreads();  // warp_sums is reused by the next call
-  return before + x - v;
-}
-
-// ---- the encoders' device scratch: a stream-ordered pool per device, kept by the library ----
-inline cudaMemPool_t scratch_pool() {
-  static std::mutex mu;
-  static std::map<int, cudaMemPool_t> pools;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
-  std::lock_guard<std::mutex> lock(mu);
-  auto it = pools.find(dev);
-  if (it != pools.end()) return it->second;
-  cudaMemPoolProps props = {};
-  props.allocType = cudaMemAllocationTypePinned;
-  props.location.type = cudaMemLocationTypeDevice;
-  props.location.id = dev;
-  cudaMemPool_t pool = nullptr;
-  if (cudaMemPoolCreate(&pool, &props) != cudaSuccess) return nullptr;
-  uint64_t keep = ~0ull;  // keep freed scratch for the next call instead of returning it at every synchronisation
-  cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-  pools[dev] = pool;
-  return pool;
-}
-
-struct Scratch {
-  cudaStream_t st;
-  std::vector<void*> held;
-  ~Scratch() {
-    for (void* p : held) cudaFreeAsync(p, st);
-  }
-  template <class T>
-  T* get(size_t count, cudaMemPool_t pool) {
-    void* p = nullptr;
-    if (cudaMallocFromPoolAsync(&p, count * sizeof(T) + 16, pool, st) != cudaSuccess) return nullptr;
-    held.push_back(p);
-    return static_cast<T*>(p);
-  }
-};
 
 }  // namespace scn

@@ -4,6 +4,7 @@ torch is used only for device memory and streams; every function below enqueues 
 sm_90a kernels from libscn_kernels.so on the current torch CUDA stream.
 """
 import ctypes
+import itertools
 
 import numpy as np
 import torch
@@ -19,6 +20,39 @@ def _need_cuda(*ts):
     for t in ts:
         if not (isinstance(t, torch.Tensor) and t.is_cuda):
             raise cabi.ScnError("scanner_b200 kernels need CUDA tensors (no CPU fallback)")
+
+
+def _per_shape(frames, run):
+    """A list of (H,W,C) uint8 CUDA tensors, shapes may differ: run(src_ptrs, h, w, c, device) on each run of
+    consecutive frames of one shape, its results concatenated in order."""
+    lst = [t.contiguous() for t in frames]
+    _need_cuda(*lst)
+    for t in lst:
+        assert t.dtype == torch.uint8 and t.dim() == 3
+    outs = []
+    for shape, group in itertools.groupby(lst, key=lambda t: t.shape):
+        group = list(group)
+        outs += list(run([t.data_ptr() for t in group], *shape, group[0].device))
+    return outs
+
+
+def _encode(name, n, device, call):
+    """call(alloc_fn, sizes) runs one scn_*_encode_u8 of n frames, which asks alloc_fn once for its whole output
+    -> list of n bytes objects.  Synchronises the current stream."""
+    keep = []
+
+    def alloc(_ctx, nbytes):
+        keep.append(torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device))
+        return keep[-1].data_ptr()
+
+    sizes = (ctypes.c_size_t * n)()
+    cabi.check(call(cabi.ALLOC_FN(alloc), sizes), name)
+    data = keep[0].cpu().numpy().tobytes()  # on the current stream, after the output is written
+    out, at = [], 0
+    for s in sizes:
+        out.append(data[at:at + s])
+        at += s
+    return out
 
 
 def histogram(frames):
@@ -204,19 +238,7 @@ def convert_color(frames, code, width=None, height=None):
         frames = frames.contiguous()
         n, h, w, c = frames.shape
         return run([frames.data_ptr() + i * h * w * c for i in range(n)], h, w, c, frames.device)
-    lst = [t.contiguous() for t in frames]
-    _need_cuda(*lst)
-    for t in lst:
-        assert t.dtype == torch.uint8 and t.dim() == 3
-    outs = []
-    i = 0
-    while i < len(lst):
-        j = i + 1
-        while j < len(lst) and lst[j].shape == lst[i].shape:
-            j += 1
-        outs += list(run([t.data_ptr() for t in lst[i:j]], *lst[i].shape, lst[i].device))
-        i = j
-    return outs
+    return _per_shape(frames, run)
 
 
 def jpeg_encode_bound(width, height, channels=3):
@@ -234,23 +256,9 @@ def jpeg_encode(frames, quality=95):
     L = cabi.lib()
 
     def run(src_ptrs, h, w, c, device):
-        keep = []
-
-        def alloc(_ctx, nbytes):
-            keep.append(torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device))
-            return keep[-1].data_ptr()
-
-        cb = cabi.ALLOC_FN(alloc)
-        sizes = (ctypes.c_size_t * len(src_ptrs))()
         sp, k1 = cabi.ptr_array(src_ptrs)
-        rc = L.scn_jpeg_encode_u8(sp, len(src_ptrs), w, h, c, int(quality), cb, None, sizes, _stream())
-        cabi.check(rc, "scn_jpeg_encode_u8")
-        data = keep[0].cpu().numpy().tobytes()  # on the current stream, after the files are written
-        out, at = [], 0
-        for s in sizes:
-            out.append(data[at:at + s])
-            at += s
-        return out
+        return _encode("scn_jpeg_encode_u8", len(src_ptrs), device, lambda cb, sizes: L.scn_jpeg_encode_u8(
+            sp, len(src_ptrs), w, h, c, int(quality), cb, None, sizes, _stream()))
 
     if isinstance(frames, torch.Tensor):
         _need_cuda(frames)
@@ -260,19 +268,7 @@ def jpeg_encode(frames, quality=95):
         if n == 0:
             return []
         return run([frames.data_ptr() + i * h * w * c for i in range(n)], h, w, c, frames.device)
-    lst = [t.contiguous() for t in frames]
-    _need_cuda(*lst)
-    for t in lst:
-        assert t.dtype == torch.uint8 and t.dim() == 3
-    outs = []
-    i = 0
-    while i < len(lst):
-        j = i + 1
-        while j < len(lst) and lst[j].shape == lst[i].shape:
-            j += 1
-        outs += run([t.data_ptr() for t in lst[i:j]], *lst[i].shape, lst[i].device)
-        i = j
-    return outs
+    return _per_shape(frames, run)
 
 
 def h264_encode_bound(width, height):
@@ -318,25 +314,10 @@ def h264_encode(frames, qp=23, keyframe_distance=120, positions=None):
         raise cabi.ScnError(f"h264_encode: {w}x{h} is beyond level 5.1 (a side over 4096 or over 36,864 macroblocks)")
     if positions is not None and len(positions) != n:
         raise cabi.ScnError(f"h264_encode: {len(positions)} positions for {n} frames")
-    keep = []
-
-    def alloc(_ctx, nbytes):
-        keep.append(torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device))
-        return keep[-1].data_ptr()
-
-    cb = cabi.ALLOC_FN(alloc)
-    sizes = (ctypes.c_size_t * n)()
     pos = None if positions is None else (ctypes.c_int * n)(*[int(p) for p in positions])
     sp, k1 = cabi.ptr_array(ptrs)
-    rc = cabi.lib().scn_h264_encode_u8(sp, n, w, h, int(qp), pos, int(keyframe_distance), cb, None, sizes,
-                                       _stream())
-    cabi.check(rc, "scn_h264_encode_u8")
-    data = keep[0].cpu().numpy().tobytes()  # on the current stream, after the access units are written
-    out, at = [], 0
-    for s in sizes:
-        out.append(data[at:at + s])
-        at += s
-    return out
+    return _encode("scn_h264_encode_u8", n, device, lambda cb, sizes: cabi.lib().scn_h264_encode_u8(
+        sp, n, w, h, int(qp), pos, int(keyframe_distance), cb, None, sizes, _stream()))
 
 
 def optical_flow_sequence(frames, workspace=None, pairs_per_call=None):

@@ -1,7 +1,7 @@
 """scn_h264_encode_u8 on the GPU, byte for byte against oracle/h264_enc.py (itself held to FFmpeg in
-tests/test_h264_encode_cpu.py): the CPU sweep, 1080p and 2160p frames, batches over 64 frames, unaligned frames.
-The engine's decoder then reads the kernel's streams back to exactly the oracle's reconstruction, chroma
-included."""
+tests/test_h264_encode_cpu.py): the CPU sweep, 1080p and 2160p frames, batches over 64 frames, unaligned frames,
+outputs pre-filled with 0x00 and 0xFF and followed by guard bytes.  The engine's decoder then reads the kernel's
+streams back to exactly the oracle's reconstruction, chroma included."""
 import ctypes
 
 import numpy as np
@@ -9,6 +9,8 @@ import pytest
 import torch
 
 import oracle
+from helpers import guarded_output
+from helpers.h264_cases import epb_seam_frames
 from oracle import h264_enc as H
 from scanner_b200 import cabi, kernels
 from scanner_b200 import engine as E
@@ -63,6 +65,30 @@ def test_unaligned_frames_equal_the_oracle():
         views.append(buf[off:off + h * w * 3].view(h, w, 3))
         views[-1].copy_(torch.from_numpy(frames[i]))
     assert kernels.h264_encode(views, 20, 2) == H.encode(frames, 20, 2)[0]
+
+
+def _encode_raw(frames, qp, kd, fill):
+    """scn_h264_encode_u8 into an output pre-filled with `fill` and followed by guard bytes (helpers.guarded_output)
+    -> the access units."""
+    frames = np.ascontiguousarray(frames)
+    n, h, w = frames.shape[:3]
+    dev = torch.from_numpy(frames).cuda()
+    pp, _keep = cabi.ptr_array([dev.data_ptr() + i * h * w * 3 for i in range(n)])
+    L = cabi.lib()
+    return guarded_output.encode_raw("scn_h264_encode_u8", n, fill, lambda cb, sizes, stream:
+                                     L.scn_h264_encode_u8(pp, n, w, h, qp, None, kd, cb, None, sizes, stream))
+
+
+@pytest.mark.parametrize("fill", [0x00, 0xFF])
+def test_prefilled_outputs_and_guards(fill):
+    """the emulation-prevention seam frames, whose payloads carry escapes at lane and chunk edges; and 70 frames at
+    keyframe_distance 3, so that IDR and non-IDR prefixes alternate within each launch and across the 64-frame
+    split"""
+    seams = epb_seam_frames()
+    assert _encode_raw(seams, 0, 120, fill) == H.encode(seams, 0)[0]
+    frames = np.random.default_rng(70).integers(0, 256, (70, 32, 48, 3), dtype=np.uint8)
+    frames[::4] //= 16
+    assert _encode_raw(frames, 27, 3, fill) == H.encode(frames, 27, 3)[0]
 
 
 def test_the_decoder_reads_the_kernels_stream_back_to_the_reconstruction():

@@ -9,13 +9,14 @@ import numpy as np
 import pytest
 import torch
 
+from helpers.h264_cases import epb_seam_frames
 from oracle import h264_enc as H
 from oracle import lavc
 from scanner_b200 import kernels
 
 pytestmark = pytest.mark.gpu
 
-LANE, CHUNK = 16, 4096   # bytes per thread and per CTA of h264_count_epb_kernel / h264_stuff_kernel
+LANE, CHUNK = 16, 4096   # bytes per thread and per CTA of the escape passes (kLane, kChunk in bitstream.cuh)
 
 
 def _decode(aus, w, h):
@@ -100,14 +101,8 @@ def _epb_pairs(rbsp):
     return out
 
 
-# 512 x 256 noise at QP 0 from these seeds, found by searching seeds 0-399 with the oracle: seed 25 puts a zero
-# pair across a lane boundary (at 58735) and across a chunk boundary (at 204799), seed 88 starts one exactly at a
-# chunk (at 28672).  The payload offsets are where the kernel's passes see them: its slice RBSP starts 16-aligned.
-EPB_SEEDS = (25, 88)
-
-
 def test_emulation_prevention_at_lane_and_chunk_seams():
-    frames = np.stack([np.random.default_rng(s).integers(0, 256, (256, 512, 3), dtype=np.uint8) for s in EPB_SEEDS])
+    frames = epb_seam_frames()
     pairs = [p for au in H.encode(frames, 0)[0] for p in _epb_pairs(_rbsp(au))]
     assert any(p % LANE == LANE - 1 and p % CHUNK != CHUNK - 1 for p in pairs), "no pair across a lane seam"
     assert any(p % CHUNK == CHUNK - 1 for p in pairs), "no pair across a chunk seam"

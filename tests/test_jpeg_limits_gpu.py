@@ -9,7 +9,6 @@
   * one-chunk frames beside frames of over a hundred chunks, in one launch and across the 64-frame split, and calls of
     very different sizes back to back on one stream;
   * the ImageEncoder op at the 65500-wide limit and one pixel past it."""
-import ctypes
 import os
 
 import numpy as np
@@ -17,6 +16,7 @@ import pytest
 import torch
 
 import scanner_b200 as sp
+from helpers import guarded_output
 from oracle import jpeg as J
 from scanner_b200 import cabi, kernels
 
@@ -24,39 +24,18 @@ pytestmark = pytest.mark.gpu
 
 CORPUS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "jpeg_symbols.npz")
 
-GUARD = 4096
-SENTINEL = 0xDEADBEEFDEADBEEF
-
 
 def encode_raw(frames, quality, fill):
-    """scn_jpeg_encode_u8 of equal-shape frames into an output pre-filled with `fill` and followed by GUARD bytes of
-    `fill`; checks what the call reports and that the guard is untouched -> the files."""
+    """scn_jpeg_encode_u8 of equal-shape frames into an output pre-filled with `fill` and followed by guard bytes
+    (helpers.guarded_output) -> the files."""
     frames = [np.ascontiguousarray(f) for f in frames]
     h, w = frames[0].shape[:2]
     c = 1 if frames[0].ndim == 2 else frames[0].shape[2]
     dev = [torch.from_numpy(f).cuda() for f in frames]
-    out = {}
-
-    def alloc(_ctx, nbytes):
-        out["n"] = int(nbytes)
-        out["buf"] = torch.full((int(nbytes) + GUARD,), fill, dtype=torch.uint8, device="cuda")
-        return out["buf"].data_ptr()
-
-    cb = cabi.ALLOC_FN(alloc)
-    sizes = (ctypes.c_size_t * len(frames))(*[SENTINEL] * len(frames))
     pp, _keep = cabi.ptr_array([t.data_ptr() for t in dev])
-    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    cabi.check(cabi.lib().scn_jpeg_encode_u8(pp, len(frames), w, h, c, quality, cb, None, sizes, stream),
-               "scn_jpeg_encode_u8")
-    data = out["buf"].cpu().numpy()
-    assert SENTINEL not in list(sizes)
-    assert out["n"] == sum(sizes)
-    assert (data[out["n"]:] == fill).all(), "bytes written past the end of the output"
-    files, at = [], 0
-    for s in sizes:
-        files.append(data[at:at + s].tobytes())
-        at += s
-    return files
+    L = cabi.lib()
+    return guarded_output.encode_raw("scn_jpeg_encode_u8", len(frames), fill, lambda cb, sizes, stream:
+                                     L.scn_jpeg_encode_u8(pp, len(frames), w, h, c, quality, cb, None, sizes, stream))
 
 
 def check(frames, quality, got, cv2=True):
