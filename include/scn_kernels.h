@@ -75,7 +75,7 @@ SCN_API int scn_hist16_u8c3_strided(const uint8_t* base, size_t stride_bytes, in
  *          including its exact-2x INTER_AREA re-route).  Bit-exact vs cv2.resize.
  *
  * scn_resize_target: the output size rule of test_ops.cpp:126-147 (ResizeArgs width, height,
- * min, preserve_aspect; `interpolation` is ignored by the reference).
+ * min, preserve_aspect; `interpolation` is ignored by the reference and selects scn_resize_interp_* below here).
  *
  * A "plan" is the per-(src size, dst size) coefficient table (x/y tap offsets and 11-bit
  * weights).  The caller owns its storage: ask for the size, fill it on the host, copy it to the
@@ -92,6 +92,42 @@ SCN_API int scn_resize_bilinear_u8c3(const uint8_t* const* host_src_ptrs, int n,
 SCN_API int scn_resize_bilinear_u8c3_strided(const uint8_t* src, size_t src_stride, int n, int src_w,
                                      int src_h, uint8_t* dst, size_t dst_stride, int dst_w,
                                      int dst_h, const void* plan, void* stream);
+
+/* Resize with ResizeArgs.interpolation (scannertools' Resize: cv::resize(img, out, Size(w,h), 0, 0,
+ * interpolation)).  Bit-exact vs cv2.resize on u8 HxWx3 frames for the modes built here, numbered as cv2's
+ * InterpolationFlags:
+ *   0 INTER_NEAREST  s = min(floor(d * scale), src - 1) per axis, scale = 1.0 / ((double)dst / src)
+ *   1 INTER_LINEAR   what scn_resize_bilinear_u8c3 computes (and, through scn_resize_interp_nv12, what
+ *                    scn_nv12_hist_resize computes), with the same plan
+ *   3 INTER_AREA     both scales integers: the box average (2 x 2 rounds half up, as INTER_LINEAR's exact-2x
+ *                    re-route; other factors round the float product half to even); both scales >= 1 otherwise:
+ *                    OpenCV's float area tables in its order of operations; a scale below 1 (an upscale on either
+ *                    axis): INTER_LINEAR's fixed-point arithmetic with INTER_AREA's taps
+ * scn_resize_interp_code: the mode of a name; "" is INTER_LINEAR.  SCN_E_UNSUPPORTED for INTER_CUBIC,
+ *   INTER_LANCZOS4, INTER_LINEAR_EXACT and INTER_NEAREST_EXACT (not built), SCN_E_BADARG for any other name.
+ * scn_resize_interp_supported: the names of the built modes, comma separated, for error messages.
+ * scn_resize_interp_plan_bytes / _plan_fill: the plan of (mode, src size, dst size), filled on the host and copied
+ *   to the device as for scn_resize_plan_fill (whose plan is the INTER_LINEAR one, byte for byte).  The size query
+ *   returns 0 for arguments the fill refuses.
+ * scn_resize_interp_u8c3: n dense RGB24 frames, any base alignment, pointer list; batches over 64 frames are split
+ *   into launches.  scn_resize_interp_nv12: n NV12 surfaces as scn_nv12_to_rgb24 takes them, identical to
+ *   scn_nv12_to_rgb24 followed by scn_resize_interp_u8c3; the RGB24 frame is never written.
+ *   A mode code other than 0, 1, 3 returns SCN_E_UNSUPPORTED (2, 4, 5, 6) or SCN_E_BADARG before any launch; so does
+ *   a destination of more than INT_MAX pixels.  A null plan is SCN_E_PLAN except at an exact 2x downscale of both
+ *   axes (INTER_LINEAR, INTER_AREA).  INTER_AREA downscales whose widest row of source columns per 256 destination
+ *   columns exceeds about 77,000 pixels return SCN_E_UNSUPPORTED (one staged row must fit in shared memory).
+ */
+SCN_API int scn_resize_interp_code(const char* name);
+SCN_API const char* scn_resize_interp_supported(void);
+SCN_API size_t scn_resize_interp_plan_bytes(int mode, int src_w, int src_h, int dst_w, int dst_h);
+SCN_API int scn_resize_interp_plan_fill(int mode, int src_w, int src_h, int dst_w, int dst_h, void* host_plan);
+SCN_API int scn_resize_interp_u8c3(int mode, const uint8_t* const* host_src_ptrs, int n, int src_w, int src_h,
+                                   uint8_t* const* host_dst_ptrs, int dst_w, int dst_h, const void* plan,
+                                   void* stream);
+SCN_API int scn_resize_interp_nv12(int mode, const uint8_t* const* host_luma_ptrs,
+                                   const uint8_t* const* host_chroma_ptrs, size_t pitch, int n, int width, int height,
+                                   uint8_t* const* host_dst_ptrs, int dst_w, int dst_h, const void* plan,
+                                   void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Blur  (replaces BlurKernel::execute, tests/test_ops.cpp:265-294: integer box filter of

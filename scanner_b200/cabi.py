@@ -30,6 +30,14 @@ SIGNATURES = {
     "scn_resize_bilinear_u8c3": (_c.c_int, [_PP, _c.c_int, _c.c_int, _c.c_int, _PP, _c.c_int, _c.c_int, _VP, _VP]),
     "scn_resize_bilinear_u8c3_strided": (_c.c_int, [_VP, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _VP,
                                                     _c.c_size_t, _c.c_int, _c.c_int, _VP, _VP]),
+    "scn_resize_interp_code": (_c.c_int, [_c.c_char_p]),
+    "scn_resize_interp_supported": (_c.c_char_p, []),
+    "scn_resize_interp_plan_bytes": (_c.c_size_t, [_c.c_int] * 5),
+    "scn_resize_interp_plan_fill": (_c.c_int, [_c.c_int] * 5 + [_VP]),
+    "scn_resize_interp_u8c3": (_c.c_int, [_c.c_int, _PP, _c.c_int, _c.c_int, _c.c_int, _PP, _c.c_int, _c.c_int, _VP,
+                                          _VP]),
+    "scn_resize_interp_nv12": (_c.c_int, [_c.c_int, _PP, _PP, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _PP,
+                                          _c.c_int, _c.c_int, _VP, _VP]),
     "scn_box_blur_u8c3": (_c.c_int, [_PP, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _PP, _VP]),
     "scn_box_blur_u8c3_strided": (_c.c_int, [_VP, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _VP, _VP]),
     "scn_nv12_to_rgb24": (_c.c_int, [_PP, _PP, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _PP, _c.c_size_t, _VP]),

@@ -131,6 +131,7 @@ class ResizeKernelGPU : public BatchedKernel {
   void new_stream(const std::vector<u8>& args) override {
     args_ = ResizeArgs();
     args_ok_ = args_.ParseFromArray(args.data(), (int)args.size());
+    mode_ = args_ok_ ? scn_resize_interp_code(args_.interpolation().c_str()) : kLinear;
   }
 
   void execute(const BatchedElements& input_columns, BatchedElements& output_columns) override {
@@ -142,6 +143,9 @@ class ResizeKernelGPU : public BatchedKernel {
       const int sw = pic_width(f0), sh = pic_height(f0);
       int tw = 0, th = 0;
       std::string why = args_ok_ ? rgb8_problem(f0) : "could not parse ResizeArgs";
+      if (why.empty() && mode_ < 0)
+        why = std::string(mode_ == SCN_E_UNSUPPORTED ? "unsupported" : "unknown") + " interpolation '" +
+              args_.interpolation() + "'; supported: " + scn_resize_interp_supported();
       if (why.empty()) {
         scn_resize_target(sw, sh, args_.width(), args_.height(), args_.min(), args_.preserve_aspect(), &tw, &th);
         if (tw <= 0 || th <= 0 || (int64_t)tw * th > INT_MAX)
@@ -161,28 +165,41 @@ class ResizeKernelGPU : public BatchedKernel {
         src.push_back(frames[i0 + i].as_const_frame()->data);
         dst.push_back(outs[i]->data);
       }
+      const void* plan = plan_for(sw, sh, tw, th);
       if (is_nv12(f0)) {
         std::vector<const u8*> chroma;
         for (const u8* p : src) chroma.push_back(p + (size_t)sw * sh);
-        SCN_CHECK(scn_nv12_hist_resize(src.data(), chroma.data(), (size_t)sw, n, sw, sh, nullptr, dst.data(), tw, th,
-                                       plan_for(sw, sh, tw, th), device_stream(device_)));
+        if (mode_ == kLinear)
+          SCN_CHECK(scn_nv12_hist_resize(src.data(), chroma.data(), (size_t)sw, n, sw, sh, nullptr, dst.data(), tw,
+                                         th, plan, device_stream(device_)));
+        else
+          SCN_CHECK(scn_resize_interp_nv12(mode_, src.data(), chroma.data(), (size_t)sw, n, sw, sh, dst.data(), tw,
+                                           th, plan, device_stream(device_)));
+      } else if (mode_ == kLinear) {
+        SCN_CHECK(scn_resize_bilinear_u8c3(src.data(), n, sw, sh, dst.data(), tw, th, plan, device_stream(device_)));
       } else {
-        SCN_CHECK(scn_resize_bilinear_u8c3(src.data(), n, sw, sh, dst.data(), tw, th, plan_for(sw, sh, tw, th),
-                                           device_stream(device_)));
+        SCN_CHECK(scn_resize_interp_u8c3(mode_, src.data(), n, sw, sh, dst.data(), tw, th, plan,
+                                         device_stream(device_)));
       }
       for (i32 i = 0; i < n; ++i) insert_frame(output_columns[0], outs[i]);
     });
   }
 
  private:
-  // coefficient tables are built on the host once per geometry and kept on the device
+  static constexpr int kLinear = 1;  // INTER_LINEAR, scn_resize_interp_code("")
+
+  // coefficient tables are built on the host once per (mode, geometry) and kept on the device
   const void* plan_for(int sw, int sh, int dw, int dh) {
-    const std::array<int, 4> key = {sw, sh, dw, dh};
+    const std::array<int, 5> key = {mode_, sw, sh, dw, dh};
     auto it = plans_.find(key);
     if (it != plans_.end()) return it->second;
-    const size_t bytes = scn_resize_plan_bytes(dw, dh);
+    const size_t bytes =
+        mode_ == kLinear ? scn_resize_plan_bytes(dw, dh) : scn_resize_interp_plan_bytes(mode_, sw, sh, dw, dh);
     std::vector<u8> host(bytes);
-    SCN_CHECK(scn_resize_plan_fill(sw, sh, dw, dh, host.data()));
+    if (mode_ == kLinear)
+      SCN_CHECK(scn_resize_plan_fill(sw, sh, dw, dh, host.data()));
+    else
+      SCN_CHECK(scn_resize_interp_plan_fill(mode_, sw, sh, dw, dh, host.data()));
     u8* dev = new_buffer(device_, bytes);
     memcpy_buffer(dev, device_, host.data(), CPU_DEVICE, bytes);
     plans_[key] = dev;
@@ -192,7 +209,8 @@ class ResizeKernelGPU : public BatchedKernel {
   DeviceHandle device_;
   ResizeArgs args_;
   bool args_ok_ = true;
-  std::map<std::array<int, 4>, u8*> plans_;
+  int mode_ = kLinear;  // a negative SCN_E_* for an interpolation name that is refused at execute()
+  std::map<std::array<int, 5>, u8*> plans_;
 };
 
 REGISTER_OP(Resize).frame_input("frame").frame_output("frame").stream_protobuf_name("ResizeArgs");

@@ -18,13 +18,22 @@ namespace {
 
 constexpr int32_t kPlanMagic = 0x5243504c;  // "LPCR"
 
-void fill_taps(int ssz, int dsz, bool zero_weight_clamp, Tap* t) {
+// cv::resize's INTER_LINEAR table for one axis; with `area`, the taps INTER_AREA uses when a scale is below 1.
+void fill_taps(int ssz, int dsz, bool zero_weight_clamp, bool area, Tap* t) {
   const double inv_scale = (double)dsz / (double)ssz;
   const double scale = 1.0 / inv_scale;
   for (int d = 0; d < dsz; ++d) {
-    float f = (float)((d + 0.5) * scale - 0.5);
-    int s = (int)floorf(f);
-    f -= (float)s;
+    float f;
+    int s;
+    if (area) {
+      s = (int)floor(d * scale);
+      f = (float)((d + 1) - (s + 1) * inv_scale);
+      f = f <= 0 ? 0.f : f - floorf(f);
+    } else {
+      f = (float)((d + 0.5) * scale - 0.5);
+      s = (int)floorf(f);
+      f -= (float)s;
+    }
     if (zero_weight_clamp) {
       // x axis: out-of-range taps collapse onto the edge pixel with weight (2048, 0)
       if (s < 0) { f = 0.f; s = 0; }
@@ -133,9 +142,7 @@ extern "C" size_t scn_resize_plan_bytes(int dst_w, int dst_h) {
   return sizeof(scn::PlanHeader) + sizeof(scn::Tap) * ((size_t)dst_w + (size_t)dst_h);
 }
 
-extern "C" int scn_resize_plan_fill(int src_w, int src_h, int dst_w, int dst_h,
-                                    void* host_plan) {
-  if (src_w <= 0 || src_h <= 0 || dst_w <= 0 || dst_h <= 0 || !host_plan) return SCN_E_BADARG;
+void scn::fill_linear_plan(int src_w, int src_h, int dst_w, int dst_h, bool area, void* host_plan) {
   scn::PlanHeader h;
   memset(&h, 0, sizeof(h));
   h.magic = scn::kPlanMagic;
@@ -144,10 +151,17 @@ extern "C" int scn_resize_plan_fill(int src_w, int src_h, int dst_w, int dst_h,
   h.dst_w = dst_w;
   h.dst_h = dst_h;
   h.area2x = (src_w == 2 * dst_w && src_h == 2 * dst_h) ? 1 : 0;
+  h.kind = scn::kPlanLinearTaps;
   memcpy(host_plan, &h, sizeof(h));
   scn::Tap* t = reinterpret_cast<scn::Tap*>((uint8_t*)host_plan + sizeof(h));
-  scn::fill_taps(src_w, dst_w, true, t);
-  scn::fill_taps(src_h, dst_h, false, t + dst_w);
+  scn::fill_taps(src_w, dst_w, true, area, t);
+  scn::fill_taps(src_h, dst_h, false, area, t + dst_w);
+}
+
+extern "C" int scn_resize_plan_fill(int src_w, int src_h, int dst_w, int dst_h,
+                                    void* host_plan) {
+  if (src_w <= 0 || src_h <= 0 || dst_w <= 0 || dst_h <= 0 || !host_plan) return SCN_E_BADARG;
+  scn::fill_linear_plan(src_w, src_h, dst_w, dst_h, false, host_plan);
   return 0;
 }
 

@@ -77,14 +77,36 @@ def histogram(frames):
     return out
 
 
-class ResizePlan:
-    """Device copy of the coefficient table for one (src size, dst size) pair."""
+def resize_interp_code(interpolation):
+    """ResizeArgs.interpolation ('', 'INTER_LINEAR', 'INTER_AREA', 'INTER_NEAREST') -> cv2's mode number.  Raises
+    for any other name, with the supported ones."""
+    L = cabi.lib()
+    code = L.scn_resize_interp_code(str(interpolation).encode())
+    if code < 0:
+        kind = "not supported" if code == -2 else "unknown"
+        raise cabi.ScnError(f"Resize interpolation {interpolation!r} is {kind}; supported: "
+                            f"{L.scn_resize_interp_supported().decode()}")
+    return code
 
-    def __init__(self, src_w, src_h, dst_w, dst_h, device="cuda"):
+
+_LINEAR = 1
+
+
+class ResizePlan:
+    """Device copy of the coefficient table for one (src size, dst size) pair and interpolation mode."""
+
+    def __init__(self, src_w, src_h, dst_w, dst_h, device="cuda", interpolation="INTER_LINEAR"):
         L = cabi.lib()
-        nbytes = L.scn_resize_plan_bytes(dst_w, dst_h)
-        host = np.zeros(nbytes, np.uint8)
-        cabi.check(L.scn_resize_plan_fill(src_w, src_h, dst_w, dst_h, host.ctypes.data), "scn_resize_plan_fill")
+        self.mode = resize_interp_code(interpolation)
+        if self.mode == _LINEAR:
+            nbytes = L.scn_resize_plan_bytes(dst_w, dst_h)
+            host = np.zeros(nbytes, np.uint8)
+            cabi.check(L.scn_resize_plan_fill(src_w, src_h, dst_w, dst_h, host.ctypes.data), "scn_resize_plan_fill")
+        else:
+            nbytes = L.scn_resize_interp_plan_bytes(self.mode, src_w, src_h, dst_w, dst_h)
+            host = np.zeros(max(nbytes, 1), np.uint8)
+            cabi.check(L.scn_resize_interp_plan_fill(self.mode, src_w, src_h, dst_w, dst_h, host.ctypes.data),
+                       "scn_resize_interp_plan_fill")
         self.host = host
         self.dev = torch.from_numpy(host).to(device)
         self.key = (src_w, src_h, dst_w, dst_h)
@@ -101,17 +123,24 @@ def resize_target(src_w, src_h, width=0, height=0, min=False, preserve_aspect=Fa
     return ow.value, oh.value
 
 
-def resize(frames, dst_w, dst_h, plan=None):
-    """frames (N,H,W,3) uint8 CUDA -> (N,dst_h,dst_w,3) uint8, OpenCV INTER_LINEAR semantics."""
+def resize(frames, dst_w, dst_h, plan=None, interpolation="INTER_LINEAR"):
+    """frames (N,H,W,3) uint8 CUDA -> (N,dst_h,dst_w,3) uint8, cv2.resize's arithmetic for `interpolation`
+    ('INTER_LINEAR' or '', 'INTER_AREA', 'INTER_NEAREST'), bit-exact."""
     _need_cuda(frames)
     frames = frames.contiguous()
     n, h, w, _ = frames.shape
-    plan = plan or ResizePlan(w, h, dst_w, dst_h, frames.device)
-    assert plan.key == (w, h, dst_w, dst_h)
+    plan = plan or ResizePlan(w, h, dst_w, dst_h, frames.device, interpolation)
+    assert plan.key == (w, h, dst_w, dst_h) and plan.mode == resize_interp_code(interpolation)
     out = torch.empty((n, dst_h, dst_w, 3), dtype=torch.uint8, device=frames.device)
-    rc = cabi.lib().scn_resize_bilinear_u8c3_strided(frames.data_ptr(), h * w * 3, n, w, h, out.data_ptr(),
-                                                     dst_h * dst_w * 3, dst_w, dst_h, plan.ptr, _stream())
-    cabi.check(rc, "scn_resize_bilinear_u8c3_strided")
+    if plan.mode == _LINEAR:
+        rc = cabi.lib().scn_resize_bilinear_u8c3_strided(frames.data_ptr(), h * w * 3, n, w, h, out.data_ptr(),
+                                                         dst_h * dst_w * 3, dst_w, dst_h, plan.ptr, _stream())
+        cabi.check(rc, "scn_resize_bilinear_u8c3_strided")
+        return out
+    sp, k1 = cabi.ptr_array([frames.data_ptr() + i * h * w * 3 for i in range(n)])
+    dp, k2 = cabi.ptr_array([out.data_ptr() + i * dst_h * dst_w * 3 for i in range(n)])
+    cabi.check(cabi.lib().scn_resize_interp_u8c3(plan.mode, sp, n, w, h, dp, dst_w, dst_h, plan.ptr, _stream()),
+               "scn_resize_interp_u8c3")
     return out
 
 
@@ -165,8 +194,11 @@ def nv12_pack(surfaces, width, height):
     return out
 
 
-def nv12_hist_resize(surfaces, width, height, dst_w, dst_h, plan=None, want_resize=True, want_hist=True):
-    """Fused configs[1] DAG on NVDEC-layout surfaces -> (hist (N,3,16) i32, resized (N,dh,dw,3) u8)."""
+def nv12_hist_resize(surfaces, width, height, dst_w, dst_h, plan=None, want_resize=True, want_hist=True,
+                     interpolation="INTER_LINEAR"):
+    """Fused configs[1] DAG on NVDEC-layout surfaces -> (hist (N,3,16) i32, resized (N,dh,dw,3) u8).  The resize
+    uses `interpolation` as resize() does; other modes than INTER_LINEAR take scn_resize_interp_nv12 (the
+    histogram then runs in a call of its own)."""
     _need_cuda(surfaces)
     surfaces = surfaces.contiguous()
     n = surfaces.shape[0]
@@ -178,10 +210,18 @@ def nv12_hist_resize(surfaces, width, height, dst_w, dst_h, plan=None, want_resi
     op = None
     pptr = None
     if want_resize:
-        plan = plan or ResizePlan(width, height, dst_w, dst_h, surfaces.device)
+        plan = plan or ResizePlan(width, height, dst_w, dst_h, surfaces.device, interpolation)
+        assert plan.key == (width, height, dst_w, dst_h) and plan.mode == resize_interp_code(interpolation)
         res = torch.empty((n, dst_h, dst_w, 3), dtype=torch.uint8, device=surfaces.device)
         op, k3 = cabi.ptr_array([res.data_ptr() + i * dst_h * dst_w * 3 for i in range(n)])
         pptr = plan.ptr
+        if plan.mode != _LINEAR:
+            rc = cabi.lib().scn_resize_interp_nv12(plan.mode, lp, cp, pitch, n, width, height, op, dst_w, dst_h,
+                                                   pptr, _stream())
+            cabi.check(rc, "scn_resize_interp_nv12")
+            if not want_hist:
+                return None, res
+            op = None
     rc = cabi.lib().scn_nv12_hist_resize(lp, cp, pitch, n, width, height, hist.data_ptr() if want_hist else None,
                                          op, dst_w, dst_h, pptr, _stream())
     cabi.check(rc, "scn_nv12_hist_resize")
