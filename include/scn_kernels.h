@@ -225,13 +225,44 @@ SCN_API int scn_convert_color_nv12(const uint8_t* const* host_luma_ptrs, const u
  * scn_jpeg_encode_bound: bytes no file of that geometry exceeds at any quality (0 for an unsupported
  *   geometry): the header, every block at its longest code (26 bits per AC coefficient, 22 for the DC),
  *   every byte stuffed, and the EOI.
+ * scn_jpeg_encode_u8_opts / scn_jpeg_encode_bound_opts: the same with cv2's other JPEG options (a null `opts`
+ *   is all zeros: the two calls above).
+ *   sampling        the luma sampling factors h << 4 | v, chroma at 1 x 1, as
+ *                   IMWRITE_JPEG_SAMPLING_FACTOR: SCN_JPEG_444 (0x11), SCN_JPEG_422 (0x21), SCN_JPEG_420 (0x22),
+ *                   SCN_JPEG_440 (0x12), SCN_JPEG_411 (0x41); 0 is 4:2:0.  Gray frames ignore it.
+ *   luma_quality,   IMWRITE_JPEG_LUMA_QUALITY / IMWRITE_JPEG_CHROMA_QUALITY, 1-100, 0 when absent, with cv2's
+ *   chroma_quality  rules: a luma quality alone scales both tables (in place of `quality`), a chroma quality alone
+ *                   is ignored, both scale each its own table, and two different ones code 4:4:4 whatever
+ *                   `sampling` says.
+ *   optimize        1: IMWRITE_JPEG_OPTIMIZE, Huffman tables built per frame from its own symbol counts
+ *                   (libjpeg's jpeg_gen_optimal_table), listed in the frame's DHT segments; 0: Annex K tables.
+ *   Any other sampling, optimize other than 0 or 1, or a quality outside 1-100: SCN_E_BADARG (the bound returns
+ *   0).  4:4:4 has twice the blocks of 4:2:0, and optimised codes can be longer, so the bound depends on the options.
+ * scn_jpeg_optimal_table: the optimised-table builder alone, on one warp (synchronous, the legacy default stream):
+ *   symbol frequencies host_freq[256] -> BITS host_bits[16] and HUFFVAL host_vals[256] (the first sum(BITS) used).
  */
 #define SCN_E_ALLOC (-4)
+#define SCN_JPEG_444 0x11
+#define SCN_JPEG_422 0x21
+#define SCN_JPEG_420 0x22
+#define SCN_JPEG_440 0x12
+#define SCN_JPEG_411 0x41
+typedef struct scn_jpeg_options {
+  int sampling;
+  int luma_quality;
+  int chroma_quality;
+  int optimize;
+} scn_jpeg_options;
 typedef void* (*scn_alloc_fn)(void* ctx, size_t bytes);
 SCN_API size_t scn_jpeg_encode_bound(int width, int height, int channels);
 SCN_API int scn_jpeg_encode_u8(const uint8_t* const* host_src_ptrs, int n, int width, int height, int channels,
                                int quality, scn_alloc_fn alloc_out, void* alloc_ctx, size_t* host_sizes,
                                void* stream);
+SCN_API size_t scn_jpeg_encode_bound_opts(int width, int height, int channels, const scn_jpeg_options* opts);
+SCN_API int scn_jpeg_encode_u8_opts(const uint8_t* const* host_src_ptrs, int n, int width, int height, int channels,
+                                    int quality, const scn_jpeg_options* opts, scn_alloc_fn alloc_out,
+                                    void* alloc_ctx, size_t* host_sizes, void* stream);
+SCN_API int scn_jpeg_optimal_table(const uint64_t* host_freq, uint8_t* host_bits, uint8_t* host_vals);
 
 /* ---------------------------------------------------------------------------------------
  * H.264  (the save stage's video encoder: upstream, compress_video() outputs went through libavcodec).

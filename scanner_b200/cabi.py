@@ -16,6 +16,14 @@ _PP = _c.POINTER(_c.c_void_p)
 # scn_alloc_fn: (ctx, bytes) -> device pointer
 ALLOC_FN = _c.CFUNCTYPE(_c.c_void_p, _c.c_void_p, _c.c_size_t)
 
+
+class JpegOptions(_c.Structure):
+    """scn_jpeg_options: sampling (luma factors h << 4 | v, 0 for 4:2:0), luma_quality, chroma_quality (0: absent),
+    optimize (0 or 1)."""
+    _fields_ = [("sampling", _c.c_int), ("luma_quality", _c.c_int), ("chroma_quality", _c.c_int),
+                ("optimize", _c.c_int)]
+
+
 # name -> (restype, argtypes); must list every symbol declared in include/scn_kernels.h
 SIGNATURES = {
     "scn_abi_version": (_c.c_int, []),
@@ -60,6 +68,10 @@ SIGNATURES = {
     "scn_jpeg_encode_bound": (_c.c_size_t, [_c.c_int, _c.c_int, _c.c_int]),
     "scn_jpeg_encode_u8": (_c.c_int, [_PP, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int, ALLOC_FN, _VP,
                                       _c.POINTER(_c.c_size_t), _VP]),
+    "scn_jpeg_encode_bound_opts": (_c.c_size_t, [_c.c_int, _c.c_int, _c.c_int, _c.c_void_p]),
+    "scn_jpeg_encode_u8_opts": (_c.c_int, [_PP, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_void_p,
+                                           ALLOC_FN, _VP, _c.POINTER(_c.c_size_t), _VP]),
+    "scn_jpeg_optimal_table": (_c.c_int, [_c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint8), _c.POINTER(_c.c_uint8)]),
     "scn_h264_encode_bound": (_c.c_size_t, [_c.c_int, _c.c_int]),
     "scn_h264_encode_u8": (_c.c_int, [_PP, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.POINTER(_c.c_int), _c.c_int,
                                       ALLOC_FN, _VP, _c.POINTER(_c.c_size_t), _VP]),

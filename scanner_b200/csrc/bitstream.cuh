@@ -10,7 +10,9 @@
 //   count(p, at, v, valid)     the escape bytes among the `valid` (1-16) bytes v at offset `at` of the stream p
 //   copy(p, at, v, valid, o)   writes those bytes with their escapes from o on and returns the end
 //   count_name, copy_name      the two launches' names (for the launch counter and scn_prof_*)
-// and the bytes around each stream: two prefixes, one chosen per frame, and a suffix.
+// and the bytes around each stream: two prefixes, one chosen per frame, and a suffix.  Or, instead of the two
+// prefixes, one prefix per frame that the measure passes leave in device memory (FramePrefixes); the host reads their
+// lengths back with the bit counts.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -130,6 +132,13 @@ struct StreamSlots {
   uint64_t chunk_off[SCN_MAX_PTRS];   // index of each frame's first chunk count
   uint64_t out_off[SCN_MAX_PTRS];     // byte offset of each frame's output
   uint8_t prefix[SCN_MAX_PTRS];       // which of the two prefixes each frame gets
+  uint16_t prefix_len[SCN_MAX_PTRS];  // with per-frame prefixes: each frame's prefix length
+};
+
+// Per-frame prefixes in device memory: frame i's at bytes + i * kMaxPrefix, len[i] bytes long (at most kMaxPrefix).
+struct FramePrefixes {
+  const uint8_t* bytes;
+  const uint32_t* len;
 };
 
 // The bytes around each frame's stream in the output.
@@ -175,18 +184,26 @@ escape_count_kernel(int i0, const __grid_constant__ StreamSlots s, const uint8_t
   }
 }
 
-template <class Rule>
+// PerFrame: each frame's prefix is at frame_prefix + j * kMaxPrefix (FramePrefixes), else one of ax's two
+template <class Rule, bool PerFrame>
 __global__ void __launch_bounds__(kChunkThreads)
 escape_copy_kernel(const __grid_constant__ StreamSlots s, const __grid_constant__ Affixes ax, const uint8_t* streams,
-                   const uint32_t* chunk_esc, uint8_t* out) {
+                   const uint32_t* chunk_esc, uint8_t* out, const uint8_t* frame_prefix) {
   const int j = blockIdx.y;
   const uint64_t bytes = s.bytes[j];
   const uint64_t at = (uint64_t)blockIdx.x * kChunk;
   if (at >= bytes) return;
   const int pre = s.prefix[j];
+  const int pre_len = PerFrame ? s.prefix_len[j] : ax.prefix_len[pre];
   uint8_t* dst = out + s.out_off[j];
-  if (blockIdx.x == 0)
-    for (int k = threadIdx.x; k < ax.prefix_len[pre]; k += blockDim.x) dst[k] = ax.prefix[pre][k];
+  if (blockIdx.x == 0) {
+    if constexpr (PerFrame) {
+      const uint8_t* pre_bytes = frame_prefix + (size_t)j * kMaxPrefix;
+      for (int k = threadIdx.x; k < pre_len; k += blockDim.x) dst[k] = pre_bytes[k];
+    } else {
+      for (int k = threadIdx.x; k < pre_len; k += blockDim.x) dst[k] = ax.prefix[pre][k];
+    }
+  }
   // escapes of the chunks before this one
   unsigned long long before = 0;
   for (uint32_t c = threadIdx.x; c < blockIdx.x; c += blockDim.x) before += chunk_esc[s.chunk_off[j] + c];
@@ -201,7 +218,7 @@ escape_copy_kernel(const __grid_constant__ StreamSlots s, const __grid_constant_
   const unsigned long long mine =
       block_exclusive_scan<unsigned long long>((unsigned long long)(valid ? Rule::count(p, i, v, valid) : 0), &total);
   if (!valid) return;
-  uint8_t* o = Rule::copy(p, i, v, valid, dst + ax.prefix_len[pre] + i + chunk_before + mine);
+  uint8_t* o = Rule::copy(p, i, v, valid, dst + pre_len + i + chunk_before + mine);
   if (i + valid == bytes)
     for (int k = 0; k < ax.suffix_len; ++k) o[k] = ax.suffix[k];
 }
@@ -209,19 +226,27 @@ escape_copy_kernel(const __grid_constant__ StreamSlots s, const __grid_constant_
 // Runs the output stage of one call of n frames.  measure() enqueues the passes that leave each frame's bit count
 // in bits[0, n) (device); emit(i0, cnt, streams, stream_off) enqueues the pass that writes frames [i0, i0 + cnt)
 // into the zeroed `streams`, frame i0 + j at byte stream_off[j].  prefix[i] picks frame i's prefix in ax; a null
-// prefix gives every frame prefix 0.  The outputs go back to back into one buffer from alloc_out, their sizes to
-// host_sizes.  Returns the first nonzero status.
+// prefix gives every frame prefix 0; frame_prefixes, when given, replace both (measure() leaves them).  The outputs
+// go back to back into one buffer from alloc_out, their sizes to host_sizes.  Returns the first nonzero status.
 template <class Rule, class Measure, class Emit>
 int run_output_stage(int n, cudaStream_t st, cudaMemPool_t pool, Scratch& s, const uint64_t* bits,
                      const uint8_t* prefix, const Affixes& ax, Measure&& measure, Emit&& emit, scn_alloc_fn alloc_out,
-                     void* alloc_ctx, size_t* host_sizes) {
+                     void* alloc_ctx, size_t* host_sizes, FramePrefixes frame_prefixes = {nullptr, nullptr}) {
   unsigned long long* escs = s.get<unsigned long long>((size_t)n, pool);
   if (!escs) return (int)cudaErrorMemoryAllocation;
   int rc = measure();
   if (rc) return rc;
   std::vector<uint64_t> host_bits((size_t)n);
+  std::vector<uint32_t> pre_len((size_t)n);
   if ((rc = (int)cudaMemcpyAsync(host_bits.data(), bits, (size_t)n * 8, cudaMemcpyDeviceToHost, st))) return rc;
+  if (frame_prefixes.bytes &&
+      (rc = (int)cudaMemcpyAsync(pre_len.data(), frame_prefixes.len, (size_t)n * 4, cudaMemcpyDeviceToHost, st)))
+    return rc;
   if ((rc = (int)cudaStreamSynchronize(st))) return rc;
+  for (int i = 0; i < n; ++i) {
+    if (!frame_prefixes.bytes) pre_len[i] = (uint32_t)ax.prefix_len[prefix ? prefix[i] : 0];
+    if (pre_len[i] > kMaxPrefix) return SCN_E_UNSUPPORTED;
+  }
 
   // the streams, 16-byte aligned, and their chunks
   std::vector<uint64_t> bytes((size_t)n), stream_off((size_t)n), chunk_off((size_t)n), out_off((size_t)n);
@@ -248,6 +273,7 @@ int run_output_stage(int n, cudaStream_t st, cudaMemPool_t pool, Scratch& s, con
       sl.chunk_off[j] = chunk_off[i0 + j];
       sl.out_off[j] = out_off[i0 + j];
       sl.prefix[j] = prefix ? prefix[i0 + j] : 0;
+      sl.prefix_len[j] = (uint16_t)pre_len[i0 + j];
     }
     return sl;
   };
@@ -270,7 +296,7 @@ int run_output_stage(int n, cudaStream_t st, cudaMemPool_t pool, Scratch& s, con
   // the outputs, back to back in the caller's buffer
   size_t out_total = 0;
   for (int i = 0; i < n; ++i) {
-    host_sizes[i] = (size_t)ax.prefix_len[prefix ? prefix[i] : 0] + bytes[i] + esc[i] + ax.suffix_len;
+    host_sizes[i] = (size_t)pre_len[i] + bytes[i] + esc[i] + ax.suffix_len;
     out_off[i] = out_total;
     out_total += host_sizes[i];
   }
@@ -278,9 +304,13 @@ int run_output_stage(int n, cudaStream_t st, cudaMemPool_t pool, Scratch& s, con
   if (!out) return SCN_E_ALLOC;
   return for_each_chunk(n, [&](int i0, int cnt) {
     const StreamSlots sl = slots(i0, cnt);
+    const uint8_t* fp = frame_prefixes.bytes ? frame_prefixes.bytes + (size_t)i0 * kMaxPrefix : nullptr;
+    const dim3 grid((unsigned)max_chunks, (unsigned)cnt);
     return launch_kernel(Rule::copy_name, st, [&] {
-      escape_copy_kernel<Rule>
-          <<<dim3((unsigned)max_chunks, (unsigned)cnt), kChunkThreads, 0, st>>>(sl, ax, streams, chunk_esc, out);
+      if (fp)
+        escape_copy_kernel<Rule, true><<<grid, kChunkThreads, 0, st>>>(sl, ax, streams, chunk_esc, out, fp);
+      else
+        escape_copy_kernel<Rule, false><<<grid, kChunkThreads, 0, st>>>(sl, ax, streams, chunk_esc, out, fp);
     });
   });
 }

@@ -2,27 +2,35 @@
 // cv2 encodes through libjpeg(-turbo) with its defaults; each step below is libjpeg's integer arithmetic
 // (oracle/jpeg.py restates the same steps in numpy and is held to cv2.imencode):
 //   colour     rgb_ycc_convert, 16-bit fixed point; gray frames are coded as they are
-//   edges      the last pixel column / row replicated out to the block grid; for 4:2:0 chroma the last pixel row
-//              is duplicated only when H is odd, ceil(H/2) rows are downsampled, then the last chroma row is
-//              replicated down to the block height
-//   4:2:0      (a + b + c + d + bias) >> 2, bias 1, 2, 1, 2, ... along each chroma row
+//   sampling   luma factors (h, v), chroma at (1, 1): 4:2:0 (2, 2) by default, or 4:4:4 (1, 1), 4:2:2 (2, 1),
+//              4:4:0 (1, 2), 4:1:1 (4, 1) (cv2's IMWRITE_JPEG_SAMPLING_FACTOR); an MCU is 8h x 8v pixels
+//   edges      the last pixel column / row replicated out to the block grid; for chroma the last pixel row is
+//              replicated out to a multiple of v, ceil(H/v) rows are downsampled, then the last chroma row is
+//              replicated down to the block height (jcprepct.c)
+//   downsample jcsample.c: 4:2:0 (a + b + c + d + bias) >> 2, bias 1, 2, 1, 2, ... along each chroma row; 4:2:2
+//              (a + b + bias) >> 1, bias 0, 1, 0, 1, ...; 4:4:0 and 4:1:1 int_downsample, (sum + 2 or 1) / 4 or 2
 //   FDCT       jpeg_fdct_islow (CONST_BITS 13, PASS1_BITS 2) on samples - 128
-//   quantise   rounded division of |coef| by 8 q, sign restored; q from the Annex K tables scaled by quality
+//   quantise   rounded division of |coef| by 8 q, sign restored; q from the Annex K tables scaled by quality, or
+//              each table by its own quality as cv2 does with IMWRITE_JPEG_LUMA_QUALITY / _CHROMA_QUALITY
 //   entropy    Annex K Huffman tables, one DC predictor per component, MCUs in row-major order; colour MCUs are
-//              Y0 Y1 Y2 Y3 Cb Cr, and Y blocks outside the ceil(W/8) x ceil(H/8) grid are dummy blocks (AC zero,
-//              the DC of the block coded before them); 1-bits pad the last byte, 0x00 follows every 0xFF.
+//              Y0 .. Y(hv-1) Cb Cr (Y in row-major order within the MCU), and Y blocks outside the
+//              ceil(W/8) x ceil(H/8) grid are dummy blocks (AC zero, the DC of the block coded before them);
+//              1-bits pad the last byte, 0x00 follows every 0xFF.
 // Five kernels per launch of at most 64 frames, every stage parallel:
-//   jpeg_mcu_kernel<C, false>  one thread per MCU: colour, downsampling, FDCT, quantisation; records every
-//                              block's quantised DC and the bit count of the MCU's AC symbols
-//   jpeg_scan_kernel           one CTA per frame: adds the DC-difference bits, scans MCU bit counts into offsets
-//   jpeg_mcu_kernel<C, true>   recomputes each MCU from the pixels and writes its bits at its offset (the words
-//                              an MCU shares with its neighbours with atomicOr)
-//   jpeg_count_ff_kernel       0xFF bytes per 4 KiB chunk of each frame's bit stream
-//   jpeg_stuff_kernel          copies each chunk with a 0x00 after every 0xFF, and places the header and EOI
+//   jpeg_mcu_kernel<C, H, V, false>  one thread per MCU: colour, downsampling, FDCT, quantisation; records
+//                                    every block's quantised DC and the bit count of the MCU's AC symbols
+//   jpeg_scan_kernel                 one CTA per frame: adds the DC-difference bits, scans MCU bit counts into
+//                                    offsets
+//   jpeg_mcu_kernel<C, H, V, true>   recomputes each MCU from the pixels and writes its bits at its offset (the
+//                                    words an MCU shares with its neighbours with atomicOr)
+//   jpeg_count_ff_kernel             0xFF bytes per 4 KiB chunk of each frame's bit stream
+//   jpeg_stuff_kernel                copies each chunk with a 0x00 after every 0xFF, and places the header and EOI
 // The last two are the output stage of bitstream.cuh with the escape rule FfStuffing; the stage also reads back
-// each frame's bit count (to size the bit streams) and its 0xFF count (to size the output).
+// each frame's bit count (to size the bit streams) and its 0xFF count (to size the output).  H, V are the luma
+// sampling factors (1, 1 for gray frames, which have no chroma and ignore the sampling option).
 #include <cuda_runtime.h>
 
+#include <type_traits>
 #include <vector>
 
 #include "bitstream.cuh"
@@ -106,11 +114,11 @@ int quant(int base, int quality) {  // jpeg_set_quality with force_baseline
   return q < 1 ? 1 : (q > 255 ? 255 : q);
 }
 
-Tables make_tables(int quality) {
+Tables make_tables(const int (&quality)[2]) {
   Tables t;
   for (int c = 0; c < 2; ++c)
     for (int i = 0; i < 64; ++i) {
-      const uint32_t d = 8u * (uint32_t)quant(c ? kChromaQ[i] : kLumaQ[i], quality);
+      const uint32_t d = 8u * (uint32_t)quant(c ? kChromaQ[i] : kLumaQ[i], quality[c]);
       t.qdiv[c][i] = (uint16_t)d;
       t.qmag[c][i] = (uint32_t)(((1ull << 32) + d - 1) / d);
     }
@@ -122,8 +130,8 @@ Tables make_tables(int quality) {
 }
 
 // SOI, APP0 (JFIF 1.01, no units, density 1 x 1), DQT per table, SOF0, DHT per table (DC0 AC0 DC1 AC1), SOS:
-// 623 bytes in colour, within the output stage's kMaxPrefix.
-std::vector<uint8_t> make_header(int w, int h, int channels, int quality) {
+// 623 bytes in colour, within the output stage's kMaxPrefix.  hv: the luma sampling factors h << 4 | v.
+std::vector<uint8_t> make_header(int w, int h, int channels, const int (&quality)[2], int hv) {
   std::vector<uint8_t> o = {0xFF, 0xD8};
   auto marker = [&](uint8_t m, const std::vector<uint8_t>& p) {
     const size_t len = p.size() + 2;
@@ -135,12 +143,12 @@ std::vector<uint8_t> make_header(int w, int h, int channels, int quality) {
   for (int t = 0; t < ntab; ++t) {
     std::vector<uint8_t> p(65);
     p[0] = (uint8_t)t;
-    for (int i = 0; i < 64; ++i) p[1 + zz_pos(i)] = (uint8_t)quant(t ? kChromaQ[i] : kLumaQ[i], quality);
+    for (int i = 0; i < 64; ++i) p[1 + zz_pos(i)] = (uint8_t)quant(t ? kChromaQ[i] : kLumaQ[i], quality[t]);
     marker(0xDB, p);
   }
   std::vector<uint8_t> sof = {8, (uint8_t)(h >> 8), (uint8_t)h, (uint8_t)(w >> 8), (uint8_t)w, (uint8_t)channels};
   if (channels == 3)
-    sof.insert(sof.end(), {1, 0x22, 0, 2, 0x11, 1, 3, 0x11, 1});
+    sof.insert(sof.end(), {1, (uint8_t)hv, 0, 2, 0x11, 1, 3, 0x11, 1});
   else
     sof.insert(sof.end(), {1, 0x11, 0});
   marker(0xC0, sof);
@@ -163,22 +171,49 @@ std::vector<uint8_t> make_header(int w, int h, int channels, int quality) {
 // ---- geometry ----
 struct Geom {
   int w, h, c;
-  int mw, mh;  // MCUs per row / column (16 x 16 for colour, 8 x 8 for gray)
+  int mw, mh;  // MCUs per row / column (8 H x 8 V for colour, 8 x 8 for gray)
   int bpm;     // blocks per MCU
+  int ny;      // Y blocks per MCU (H V)
   int bw, bh;  // real Y blocks per row / column
-  int ch_rows; // rows of the downsampled chroma planes before replication (ceil(H / 2))
+  int ch_rows; // rows of the downsampled chroma planes before replication (ceil(H / V))
   __host__ __device__ uint32_t mcus() const { return (uint32_t)mw * (uint32_t)mh; }
 };
 
-Geom make_geom(int w, int h, int c) {
+// hv: the luma sampling factors h << 4 | v (0x11 for gray frames)
+Geom make_geom(int w, int h, int c, int hv) {
   Geom g;
   g.w = w, g.h = h, g.c = c;
-  const int m = c == 3 ? 16 : 8;
-  g.mw = (w + m - 1) / m, g.mh = (h + m - 1) / m;
-  g.bpm = c == 3 ? 6 : 1;
+  const int sh = hv >> 4, sv = hv & 15;
+  g.mw = (w + 8 * sh - 1) / (8 * sh), g.mh = (h + 8 * sv - 1) / (8 * sv);
+  g.ny = sh * sv;
+  g.bpm = c == 3 ? g.ny + 2 : 1;
   g.bw = (w + 7) / 8, g.bh = (h + 7) / 8;
-  g.ch_rows = (h + 1) / 2;
+  g.ch_rows = (h + sv - 1) / sv;
   return g;
+}
+
+// The encoder's settings after cv2's rules (grfmt_jpeg.cpp, probed on cv2 4.13): a luma quality alone sets both
+// tables, a chroma quality alone is ignored, both together scale each table by its own, and two different ones
+// force 4:4:4 whatever the sampling option says.  Gray frames have one table and no chroma: luma quality (or
+// quality) and 1 x 1.  False for an unknown sampling or a quality outside 1-100.
+struct Settings {
+  int quality[2];  // luma, chroma table
+  int hv;          // luma sampling factors h << 4 | v
+};
+
+bool settings(int channels, int quality, const scn_jpeg_options* o, Settings* s) {
+  const scn_jpeg_options none = {0, 0, 0, 0};
+  if (!o) o = &none;
+  const int hv = o->sampling ? o->sampling : 0x22;
+  if (hv != 0x11 && hv != 0x21 && hv != 0x22 && hv != 0x12 && hv != 0x41) return false;
+  for (int q : {quality, o->luma_quality, o->chroma_quality})
+    if (q < 0 || q > 100) return false;
+  if (quality < 1 || o->optimize < 0 || o->optimize > 1) return false;
+  const int lq = o->luma_quality ? o->luma_quality : quality;
+  const int cq = o->luma_quality && o->chroma_quality ? o->chroma_quality : lq;
+  s->quality[0] = lq, s->quality[1] = cq;
+  s->hv = channels != 3 ? 0x11 : (lq != cq ? 0x11 : hv);
+  return true;
 }
 
 // ---- one block: samples -> FDCT -> quantised coefficients in zig-zag order (shared memory) ----
@@ -220,20 +255,48 @@ __device__ __forceinline__ void load_luma(const uint8_t* __restrict__ src, const
   }
 }
 
-// the Cb or Cr block of MCU (mx, my): h2v2 downsampling with libjpeg's edge handling
-template <int K>
+// the Cb or Cr block of MCU (mx, my) with luma factors H, V: jcsample.c's downsampling with libjpeg's edge
+// handling (the sum of the H x V pixels under each chroma sample, then h2v2, h2v1 or int_downsample's rounding)
+template <int K, int H, int V>
 __device__ __forceinline__ void load_chroma(const uint8_t* __restrict__ src, const Geom& g, int mx, int my,
                                             int16_t* zz) {
+  if constexpr (H == 2 && V == 2) {  // the default, written out
+#pragma unroll 1
+    for (int r = 0; r < 8; ++r) {
+      const int cy = min(8 * my + r, g.ch_rows - 1);
+      const uint8_t* r0 = src + (size_t)(2 * cy) * g.w * 3;
+      const uint8_t* r1 = src + (size_t)min(2 * cy + 1, g.h - 1) * g.w * 3;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        const size_t x0 = (size_t)min(16 * mx + 2 * c, g.w - 1) * 3;
+        const size_t x1 = (size_t)min(16 * mx + 2 * c + 1, g.w - 1) * 3;
+        const int s = chroma<K>(r0 + x0) + chroma<K>(r0 + x1) + chroma<K>(r1 + x0) + chroma<K>(r1 + x1);
+        zz[(8 * r + c) * kThreads] = (int16_t)(((s + 1 + (c & 1)) >> 2) - 128);
+      }
+    }
+    return;
+  }
 #pragma unroll 1
   for (int r = 0; r < 8; ++r) {
     const int cy = min(8 * my + r, g.ch_rows - 1);
-    const uint8_t* r0 = src + (size_t)(2 * cy) * g.w * 3;
-    const uint8_t* r1 = src + (size_t)min(2 * cy + 1, g.h - 1) * g.w * 3;
+    const uint8_t* rows[V];
+    rows[0] = src + (size_t)(V * cy) * g.w * 3;  // V cy <= H - 1 as cy < ceil(H / V)
+#pragma unroll
+    for (int dy = 1; dy < V; ++dy) rows[dy] = src + (size_t)min(V * cy + dy, g.h - 1) * g.w * 3;
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
-      const size_t x0 = (size_t)min(16 * mx + 2 * c, g.w - 1) * 3, x1 = (size_t)min(16 * mx + 2 * c + 1, g.w - 1) * 3;
-      const int s = chroma<K>(r0 + x0) + chroma<K>(r0 + x1) + chroma<K>(r1 + x0) + chroma<K>(r1 + x1);
-      zz[(8 * r + c) * kThreads] = (int16_t)(((s + 1 + (c & 1)) >> 2) - 128);
+      int s = 0;
+#pragma unroll
+      for (int dx = 0; dx < H; ++dx) {
+        const size_t x = (size_t)min(8 * H * mx + H * c + dx, g.w - 1) * 3;
+#pragma unroll
+        for (int dy = 0; dy < V; ++dy) s += chroma<K>(rows[dy] + x);
+      }
+      int v;
+      if constexpr (H == 1 && V == 1) v = s;                              // fullsize_downsample
+      else if constexpr (H == 2 && V == 1) v = (s + (c & 1)) >> 1;        // h2v1_downsample
+      else v = (s + H * V / 2) / (H * V);                                 // int_downsample
+      zz[(8 * r + c) * kThreads] = (int16_t)(v - 128);
     }
   }
 }
@@ -296,9 +359,11 @@ __device__ __forceinline__ uint64_t fdct_quant(const uint32_t* qmag, const uint1
 
 __device__ __forceinline__ int bit_length(int v) { return 32 - __clz(abs(v)); }
 
-// bits of the AC symbols of one block (zz in shared memory, nz its nonzero AC mask); with W, also writes them
-template <bool Emit>
-__device__ __forceinline__ uint32_t code_ac(const int16_t* zz, uint64_t nz, const uint32_t* ac, BitWriter* bw) {
+// bits of the AC symbols of one block (zz in shared memory, nz its nonzero AC mask); with Emit, also writes them;
+// with Count, also adds each symbol to hist (shared memory)
+template <bool Emit, bool Count = false>
+__device__ __forceinline__ uint32_t code_ac(const int16_t* zz, uint64_t nz, const uint32_t* ac, BitWriter* bw,
+                                            uint32_t* hist = nullptr) {
   uint32_t bits = 0;
   int prev = 0;
   while (nz) {
@@ -309,8 +374,10 @@ __device__ __forceinline__ uint32_t code_ac(const int16_t* zz, uint64_t nz, cons
     const int nb = bit_length(v);
     for (; run > 15; run -= 16) {
       if (Emit) bw->put(ac[0xF0] >> 8, ac[0xF0] & 0xFF);
+      if (Count) atomicAdd(hist + 0xF0, 1u);
       bits += ac[0xF0] & 0xFF;
     }
+    if (Count) atomicAdd(hist + ((run << 4) | nb), 1u);
     const uint32_t sym = ac[(run << 4) | nb];
     if (Emit) bw->put(((sym >> 8) << nb) | ((uint32_t)(v < 0 ? v - 1 : v) & ((1u << nb) - 1)), (int)(sym & 0xFF) + nb);
     bits += (sym & 0xFF) + nb;
@@ -318,6 +385,7 @@ __device__ __forceinline__ uint32_t code_ac(const int16_t* zz, uint64_t nz, cons
   }
   if (prev != 63) {
     if (Emit) bw->put(ac[0] >> 8, ac[0] & 0xFF);
+    if (Count) atomicAdd(hist, 1u);
     bits += ac[0] & 0xFF;
   }
   return bits;
@@ -329,17 +397,24 @@ __device__ __forceinline__ void code_dc(int diff, const uint32_t* dc, BitWriter&
   bw.put(((sym >> 8) << nb) | ((uint32_t)(diff < 0 ? diff - 1 : diff) & ((1u << nb) - 1)), (int)(sym & 0xFF) + nb);
 }
 
-// block b of MCU m: table (0 luma, 1 chroma) and the index in dcs of the DC its difference is taken against (-1: 0)
-__device__ __forceinline__ int64_t prev_dc_index(int bpm, uint32_t m, int b) {
-  if (bpm == 1) return (int64_t)m - 1;
-  if (b >= 1 && b <= 3) return (int64_t)m * 6 + b - 1;
+// block b of MCU m (bpm blocks, the first ny of them Y): the index in dcs of the DC its difference is taken against
+// (-1: 0)
+__device__ __forceinline__ int64_t prev_dc_index(int bpm, int ny, uint32_t m, int b) {
+  if (b >= 1 && b < ny) return (int64_t)m * bpm + b - 1;
   if (m == 0) return -1;
-  return (int64_t)(m - 1) * 6 + (b == 0 ? 3 : b);
+  return (int64_t)(m - 1) * bpm + (b == 0 ? ny - 1 : b);
 }
 
 struct MeasureOut {
   int16_t* dc;      // [frame][mcu][bpm] quantised DC (a dummy block holds its predecessor's)
   uint32_t* acbits; // [frame][mcu] bits of the MCU's AC symbols
+};
+// Optimised Huffman tables: the symbol counts the statistics pass gathers and the codes built from them, per frame
+constexpr int kCodeWords = 2 * 12 + 2 * 256;  // Tables::dc and Tables::ac
+constexpr int kCodeWord0 = (int)(offsetof(Tables, dc) / 4);
+struct FrameTables {
+  const uint32_t* codes;  // [frame][kCodeWords] in Tables' dc, ac layout; null: the Annex K tables of `tables`
+  uint32_t* ac_hist;      // [frame][table][256] AC symbol counts (the statistics pass adds to them)
 };
 struct EmitIn {
   const int16_t* dc;
@@ -349,25 +424,19 @@ struct EmitIn {
   uint64_t stream_off[SCN_MAX_PTRS];  // byte offset of each frame's stream in `streams` (a multiple of 16)
 };
 
-// One thread per MCU.  !Emit: records DCs and AC bit counts.  Emit: writes the MCU's bits.
-template <int C, bool Emit>
-__global__ void __launch_bounds__(kThreads)
-jpeg_mcu_kernel(PtrBatch srcs, int i0, Geom g, const __grid_constant__ Tables tables, MeasureOut mo,
-                const __grid_constant__ EmitIn ei) {
-  __shared__ Tables t;
-  __shared__ int16_t zzs[64 * kThreads];
-  for (int i = threadIdx.x; i < (int)(sizeof(Tables) / 4); i += kThreads)
-    reinterpret_cast<uint32_t*>(&t)[i] = reinterpret_cast<const uint32_t*>(&tables)[i];
-  __syncthreads();
-  const uint32_t m = blockIdx.x * kThreads + threadIdx.x;
+enum { kMeasure, kEmit, kStats };
+
+// The work of the thread of MCU m (see jpeg_mcu_kernel).
+template <int C, int H, int V, int Mode>
+__device__ __forceinline__ void mcu_body(const PtrBatch& srcs, const Geom& g, uint32_t m, int f, const Tables& t,
+                                         int16_t* zzs, const MeasureOut& mo, const EmitIn& ei, uint32_t* hist) {
+  constexpr bool Emit = Mode == kEmit, Stats = Mode == kStats;
   const uint32_t nm = g.mcus();
-  if (m >= nm) return;
-  const int f = i0 + (int)blockIdx.y;
   const uint8_t* __restrict__ src = srcs.p[blockIdx.y];
   const int mx = (int)(m % (uint32_t)g.mw), my = (int)(m / (uint32_t)g.mw);
   int16_t* zz = zzs + threadIdx.x;
   const size_t rec = (size_t)f * nm + m;
-  constexpr int bpm = C == 3 ? 6 : 1;
+  constexpr int ny = H * V, bpm = C == 3 ? ny + 2 : 1;
   int16_t* dcs = Emit ? nullptr : mo.dc + (size_t)f * nm * bpm;
   const int16_t* dcr = Emit ? ei.dc + (size_t)f * nm * bpm : nullptr;
 
@@ -377,18 +446,18 @@ jpeg_mcu_kernel(PtrBatch srcs, int i0, Geom g, const __grid_constant__ Tables ta
   int16_t last_dc = 0;
 #pragma unroll 1
   for (int b = 0; b < bpm; ++b) {
-    const int tab = b < 4 ? 0 : 1;
+    const int tab = b < ny ? 0 : 1;
     bool real = true;
     if constexpr (C == 1) {
       load_luma<1>(src, g, mx, my, zz);
-    } else if (b < 4) {
-      const int bx = 2 * mx + (b & 1), by = 2 * my + (b >> 1);
+    } else if (b < ny) {
+      const int bx = H * mx + b % H, by = V * my + b / H;
       real = bx < g.bw && by < g.bh;
       if (real) load_luma<3>(src, g, bx, by, zz);
-    } else if (b == 4) {
-      load_chroma<1>(src, g, mx, my, zz);
+    } else if (b == ny) {
+      load_chroma<1, H, V>(src, g, mx, my, zz);
     } else {
-      load_chroma<2>(src, g, mx, my, zz);
+      load_chroma<2, H, V>(src, g, mx, my, zz);
     }
     uint64_t nz = 0;
     int16_t dc = last_dc;  // a dummy block's DC is its predecessor's
@@ -397,13 +466,13 @@ jpeg_mcu_kernel(PtrBatch srcs, int i0, Geom g, const __grid_constant__ Tables ta
       dc = zz[0];
     }
     if constexpr (Emit) {
-      const int64_t p = prev_dc_index(bpm, m, b);
+      const int64_t p = prev_dc_index(bpm, ny, m, b);
       code_dc(dc - (p < 0 ? 0 : dcr[p]), t.dc[tab], bw);
     } else {
       dcs[(size_t)m * bpm + b] = dc;
     }
-    if (real) acbits += code_ac<Emit>(zz, nz, t.ac[tab], &bw);
-    else acbits += code_ac<Emit>(zz, 0, t.ac[tab], &bw);  // EOB
+    if (real) acbits += code_ac<Emit, Stats>(zz, nz, t.ac[tab], &bw, hist + 256 * tab);
+    else acbits += code_ac<Emit, Stats>(zz, 0, t.ac[tab], &bw, hist + 256 * tab);  // EOB
     last_dc = dc;
   }
   if constexpr (Emit) {
@@ -417,14 +486,54 @@ jpeg_mcu_kernel(PtrBatch srcs, int i0, Geom g, const __grid_constant__ Tables ta
   }
 }
 
-// One CTA per frame: MCU bit counts (AC bits + DC difference bits) -> bit offsets, and the frame's total.
-__global__ void __launch_bounds__(1024)
-jpeg_scan_kernel(int i0, uint32_t nm, int bpm, Tables tables, const int16_t* dcs_all, const uint32_t* acbits_all,
-                 uint64_t* mcu_bit_all, uint64_t* total) {
-  __shared__ uint32_t dclen[2][12];
-  if (threadIdx.x < 24) dclen[threadIdx.x / 12][threadIdx.x % 12] = tables.dc[threadIdx.x / 12][threadIdx.x % 12] & 0xFF;
+// One thread per MCU.  kMeasure: records DCs and AC bit counts.  kEmit: writes the MCU's bits.  kStats: records
+// DCs and counts the AC symbols of each table, in shared memory per CTA and then into ft.ac_hist.  PerFrame: the
+// Huffman codes are this frame's (ft.codes) instead of those of `tables` (a separate instance, so that the Annex K
+// kernels carry nothing of it).
+template <int C, int H, int V, int Mode, bool PerFrame>
+__global__ void __launch_bounds__(kThreads)
+jpeg_mcu_kernel(PtrBatch srcs, int i0, Geom g, const __grid_constant__ Tables tables, MeasureOut mo,
+                const __grid_constant__ EmitIn ei, FrameTables ft) {
+  constexpr bool Stats = Mode == kStats;
+  __shared__ Tables t;
+  __shared__ int16_t zzs[64 * kThreads];
+  __shared__ uint32_t hist[Stats ? 2 * 256 : 1];
+  const int f = i0 + (int)blockIdx.y;
+  for (int i = threadIdx.x; i < (int)(sizeof(Tables) / 4); i += kThreads)
+    reinterpret_cast<uint32_t*>(&t)[i] = reinterpret_cast<const uint32_t*>(&tables)[i];
+  if constexpr (Stats)
+    for (int i = threadIdx.x; i < 2 * 256; i += kThreads) hist[i] = 0;
   __syncthreads();
+  if constexpr (PerFrame) {  // this frame's codes over the Annex K ones
+    for (int i = threadIdx.x; i < kCodeWords; i += kThreads)
+      reinterpret_cast<uint32_t*>(&t)[kCodeWord0 + i] = ft.codes[(size_t)f * kCodeWords + i];
+    __syncthreads();
+  }
+  const uint32_t m = blockIdx.x * kThreads + threadIdx.x;
+  const uint32_t nm = g.mcus();
+  if constexpr (Stats) {
+    if (m < nm) mcu_body<C, H, V, Mode>(srcs, g, m, f, t, zzs, mo, ei, hist);
+    __syncthreads();
+    uint32_t* out = ft.ac_hist + (size_t)f * 2 * 256;
+    for (int i = threadIdx.x; i < 2 * 256; i += kThreads)
+      if (hist[i]) atomicAdd(out + i, hist[i]);
+  } else {
+    if (m >= nm) return;
+    mcu_body<C, H, V, Mode>(srcs, g, m, f, t, zzs, mo, ei, hist);
+  }
+}
+
+// One CTA per frame: MCU bit counts (AC bits + DC difference bits) -> bit offsets, and the frame's total.  codes:
+// per-frame tables (FrameTables::codes), or null for those of `tables`.
+__global__ void __launch_bounds__(1024)
+jpeg_scan_kernel(int i0, uint32_t nm, int bpm, int ny, Tables tables, const uint32_t* codes, const int16_t* dcs_all,
+                 const uint32_t* acbits_all, uint64_t* mcu_bit_all, uint64_t* total) {
+  __shared__ uint32_t dclen[2][12];
   const int f = i0 + (int)blockIdx.x;
+  if (threadIdx.x < 24)
+    dclen[threadIdx.x / 12][threadIdx.x % 12] =
+        (codes ? codes[(size_t)f * kCodeWords + threadIdx.x] : tables.dc[threadIdx.x / 12][threadIdx.x % 12]) & 0xFF;
+  __syncthreads();
   const int16_t* dcs = dcs_all + (size_t)f * nm * bpm;
   const uint32_t* acbits = acbits_all + (size_t)f * nm;
   uint64_t* mcu_bit = mcu_bit_all + (size_t)f * nm;
@@ -433,9 +542,9 @@ jpeg_scan_kernel(int i0, uint32_t nm, int bpm, Tables tables, const int16_t* dcs
   auto mcu_bits = [&](uint32_t m) {
     uint64_t bits = acbits[m];
     for (int b = 0; b < bpm; ++b) {
-      const int64_t p = prev_dc_index(bpm, m, b);
+      const int64_t p = prev_dc_index(bpm, ny, m, b);
       const int nb = bit_length(dcs[(size_t)m * bpm + b] - (p < 0 ? 0 : dcs[p]));
-      bits += dclen[b < 4 ? 0 : 1][nb] + nb;
+      bits += dclen[b < ny ? 0 : 1][nb] + nb;
     }
     return bits;
   };
@@ -448,6 +557,160 @@ jpeg_scan_kernel(int i0, uint32_t nm, int bpm, Tables tables, const int16_t* dcs
     off += mcu_bits(m);
   }
   if (threadIdx.x == 0) total[f] = all;
+}
+
+// ---- optimised Huffman tables ----
+// Per frame and table, what the header's DHT segments carry: BITS[1..16] and HUFFVAL, for the DC and the AC table.
+struct HuffOut {
+  uint8_t bits[2][16];    // [class: 0 DC, 1 AC]
+  uint8_t vals[2][256];
+  int nvals[2];
+};
+
+// jpeg_gen_optimal_table (jchuff.c) on one warp: freq[0..256] (freq[256] is set to 1 here: the reserved code point
+// that keeps any code from being all 1-bits) -> o's bits and vals for class cls, and code[symbol] = code << 8 | length
+// (0 for a symbol that does not occur).  The two smallest nonzero frequencies are merged until one is left; ties go to
+// the larger index (libjpeg's "<=" scan), the second pick excludes the first.  Lengths over 16 are folded back by the
+// K.3 adjust loop; HUFFVAL lists the symbols by their unadjusted length, then by value.  Lane 0 does the list walks,
+// the warp the minimum searches.  freq, codesize and others are this warp's shared scratch.
+__device__ void gen_optimal_table(uint64_t* freq, int* codesize, int* others, HuffOut* o, int cls, uint32_t* code,
+                                  int ncode) {
+  const int lane = threadIdx.x & 31;
+  for (int i = lane; i < 257; i += 32) codesize[i] = 0, others[i] = -1;
+  if (lane == 0) freq[256] = 1;
+  __syncwarp();
+  auto pick = [&](int exclude) {  // the smallest nonzero frequency, the largest index among equals; -1: none
+    unsigned long long best = ~0ull;
+    for (int i = lane; i < 257; i += 32)
+      if (freq[i] && i != exclude) {
+        const unsigned long long key = (unsigned long long)freq[i] << 9 | (unsigned)(511 - i);
+        best = key < best ? key : best;
+      }
+#pragma unroll
+    for (int d = 16; d; d >>= 1) {
+      const unsigned long long y = __shfl_xor_sync(0xFFFFFFFFu, best, d);
+      best = y < best ? y : best;
+    }
+    return best == ~0ull ? -1 : 511 - (int)(best & 511);
+  };
+  for (;;) {
+    int c1 = pick(-1);
+    int c2 = pick(c1);
+    if (c2 < 0) break;
+    if (lane == 0) {
+      freq[c1] += freq[c2];
+      freq[c2] = 0;
+      ++codesize[c1];
+      while (others[c1] >= 0) c1 = others[c1], ++codesize[c1];
+      others[c1] = c2;
+      ++codesize[c2];
+      while (others[c2] >= 0) c2 = others[c2], ++codesize[c2];
+    }
+    __syncwarp();
+  }
+  if (lane == 0) {
+    int bits[33] = {0};
+    for (int i = 0; i < 257; ++i)  // libjpeg refuses lengths over 32 (Fibonacci-like counts of over 9 M)
+      if (codesize[i]) ++bits[min(codesize[i], 32)];
+    for (int i = 32; i > 16; --i)
+      while (bits[i] > 0) {
+        int j = i - 2;
+        while (bits[j] == 0) --j;
+        bits[i] -= 2;
+        ++bits[i - 1];
+        bits[j + 1] += 2;
+        --bits[j];
+      }
+    int i = 16;
+    while (i > 0 && bits[i] == 0) --i;
+    if (i > 0) --bits[i];  // the reserved code point
+    int n = 0;
+    for (int len = 1; len <= 32; ++len)
+      for (int j = 0; j < 256; ++j)
+        if (codesize[j] == len) o->vals[cls][n++] = (uint8_t)j;
+    o->nvals[cls] = n;
+    for (int k = 0; k < ncode; ++k) code[k] = 0;
+    uint32_t c = 0;
+    int k = 0;
+    for (int len = 1; len <= 16; ++len) {
+      o->bits[cls][len - 1] = (uint8_t)bits[len];
+      for (int j = 0; j < bits[len]; ++j) code[o->vals[cls][k++]] = c++ << 8 | (uint32_t)len;
+      c <<= 1;
+    }
+  }
+  __syncwarp();
+}
+
+// The bytes of each frame's header: SOI, APP0, DQT and SOF0 (head), the four DHT segments of its tables, SOS.
+struct HeaderParts {
+  uint8_t head[kMaxPrefix];
+  uint8_t sos[16];
+  int head_len, sos_len, ntab;
+};
+
+// One CTA of two warps per frame: warp t counts the DC categories of table t's blocks from the recorded DCs, then
+// builds table t's DC and AC codes from those counts and the statistics pass's AC counts (gen_optimal_table).  Then
+// thread 0 writes the frame's header to prefix[frame] (kMaxPrefix bytes per frame) and its length to prefix_len.
+__global__ void __launch_bounds__(64)
+jpeg_table_kernel(int i0, uint32_t nm, int bpm, int ny, const int16_t* dcs_all, const uint32_t* ac_hist,
+                  uint32_t* codes, uint8_t* prefix, uint32_t* prefix_len, const __grid_constant__ HeaderParts hp) {
+  __shared__ uint64_t freq[2][257];
+  __shared__ int codesize[2][257], others[2][257];
+  __shared__ uint32_t dccount[2][12];
+  __shared__ HuffOut out[2];
+  const int f = i0 + (int)blockIdx.x, t = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint32_t* code = codes + (size_t)f * kCodeWords;
+  if (lane < 12) dccount[t][lane] = 0;
+  __syncwarp();
+  if (t < hp.ntab) {
+    const int16_t* dcs = dcs_all + (size_t)f * nm * bpm;
+    const uint64_t blocks = (uint64_t)nm * bpm;
+    for (uint64_t i = lane; i < blocks; i += 32) {
+      const uint32_t m = (uint32_t)(i / bpm);
+      const int b = (int)(i - (uint64_t)m * bpm);
+      if ((b < ny ? 0 : 1) != t) continue;
+      const int64_t p = prev_dc_index(bpm, ny, m, b);
+      atomicAdd(&dccount[t][bit_length(dcs[i] - (p < 0 ? 0 : dcs[p]))], 1u);
+    }
+    __syncwarp();
+    for (int i = lane; i < 257; i += 32) freq[t][i] = i < 12 ? dccount[t][i] : 0;
+    __syncwarp();
+    gen_optimal_table(freq[t], codesize[t], others[t], &out[t], 0, code + 12 * t, 12);
+    const uint32_t* h = ac_hist + ((size_t)f * 2 + t) * 256;
+    for (int i = lane; i < 257; i += 32) freq[t][i] = i < 256 ? h[i] : 0;
+    __syncwarp();
+    gen_optimal_table(freq[t], codesize[t], others[t], &out[t], 1, code + 24 + 256 * t, 256);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint8_t* o = prefix + (size_t)f * kMaxPrefix;
+    int n = 0;
+    for (int k = 0; k < hp.head_len; ++k) o[n++] = hp.head[k];
+    for (int tab = 0; tab < hp.ntab; ++tab)
+      for (int cls = 0; cls < 2; ++cls) {
+        const int len = 2 + 1 + 16 + out[tab].nvals[cls];
+        o[n++] = 0xFF, o[n++] = 0xC4, o[n++] = (uint8_t)(len >> 8), o[n++] = (uint8_t)len;
+        o[n++] = (uint8_t)(cls << 4 | tab);
+        for (int k = 0; k < 16; ++k) o[n++] = out[tab].bits[cls][k];
+        for (int k = 0; k < out[tab].nvals[cls]; ++k) o[n++] = out[tab].vals[cls][k];
+      }
+    for (int k = 0; k < hp.sos_len; ++k) o[n++] = hp.sos[k];
+    prefix_len[f] = (uint32_t)n;
+  }
+}
+
+// One warp: gen_optimal_table of 257 given frequencies (freq[256] ignored) -> bits, vals, nvals (test entry point)
+__global__ void jpeg_gen_table_kernel(const uint64_t* freq_in, uint8_t* bits, uint8_t* vals, int* nvals) {
+  __shared__ uint64_t freq[257];
+  __shared__ int codesize[257], others[257];
+  __shared__ HuffOut out;
+  __shared__ uint32_t code[256];
+  for (int i = threadIdx.x; i < 257; i += 32) freq[i] = i < 256 ? freq_in[i] : 0;
+  __syncwarp();
+  gen_optimal_table(freq, codesize, others, &out, 0, code, 256);
+  for (int i = threadIdx.x; i < 256; i += 32) vals[i] = out.vals[0][i];
+  if (threadIdx.x < 16) bits[threadIdx.x] = out.bits[0][threadIdx.x];
+  if (threadIdx.x == 0) *nvals = out.nvals[0];
 }
 
 // B.1.1.5: a 0x00 after every 0xFF of the scan
@@ -472,25 +735,66 @@ struct FfStuffing {
   }
 };
 
-size_t worst_bits_per_block() { return 11 + 11 + 63 * (16 + 10); }  // DC code + value, 63 AC codes + values
+// DC code + value, 63 AC codes + values: Annex K codes are at most 11 (DC) and 16 (AC) bits, optimised ones 16
+size_t worst_bits_per_block(bool optimize) { return (optimize ? 16 : 11) + 11 + 63 * (16 + 10); }
+
+// jpeg_mcu_kernel for the channels and luma sampling factors of one call
+template <int Mode>
+void launch_mcu(int channels, int hv, dim3 grid, cudaStream_t st, const PtrBatch& src, int i0, const Geom& g,
+                const Tables& tables, const MeasureOut& mo, const EmitIn& ei, const FrameTables& ft) {
+  constexpr bool kOpt = Mode != kStats;  // the statistics pass codes nothing, so it needs no per-frame codes
+  auto pick = [&](auto per_frame) {
+    constexpr bool P = decltype(per_frame)::value;
+    auto k = jpeg_mcu_kernel<1, 1, 1, Mode, P>;
+    if (channels == 3) {
+      switch (hv) {
+        case 0x11: k = jpeg_mcu_kernel<3, 1, 1, Mode, P>; break;
+        case 0x21: k = jpeg_mcu_kernel<3, 2, 1, Mode, P>; break;
+        case 0x12: k = jpeg_mcu_kernel<3, 1, 2, Mode, P>; break;
+        case 0x41: k = jpeg_mcu_kernel<3, 4, 1, Mode, P>; break;
+        default: k = jpeg_mcu_kernel<3, 2, 2, Mode, P>; break;
+      }
+    }
+    k<<<grid, kThreads, 0, st>>>(src, i0, g, tables, mo, ei, ft);
+  };
+  if constexpr (kOpt) {
+    if (ft.codes) return pick(std::true_type{});
+  }
+  pick(std::false_type{});
+}
 
 }  // namespace
 }  // namespace scn
 
 extern "C" size_t scn_jpeg_encode_bound(int width, int height, int channels) {
+  return scn_jpeg_encode_bound_opts(width, height, channels, nullptr);
+}
+
+extern "C" size_t scn_jpeg_encode_bound_opts(int width, int height, int channels, const scn_jpeg_options* opts) {
   using namespace scn;
   if (width <= 0 || height <= 0 || width > kMaxDim || height > kMaxDim || (channels != 1 && channels != 3)) return 0;
-  const Geom g = make_geom(width, height, channels);
+  Settings set;
+  if (!settings(channels, 95, opts, &set)) return 0;
+  const Geom g = make_geom(width, height, channels, set.hv);
   const size_t blocks = (size_t)g.mcus() * g.bpm;
-  const size_t bytes = (blocks * worst_bits_per_block() + 7) / 8;
-  return make_header(width, height, channels, 95).size() + 2 * bytes + 2;
+  const size_t bytes = (blocks * worst_bits_per_block(opts && opts->optimize) + 7) / 8;
+  // the Annex K tables list every DC and AC symbol, so no optimised header is longer
+  return make_header(width, height, channels, set.quality, set.hv).size() + 2 * bytes + 2;
 }
 
 extern "C" int scn_jpeg_encode_u8(const uint8_t* const* host_src_ptrs, int n, int width, int height, int channels,
                                   int quality, scn_alloc_fn alloc_out, void* alloc_ctx, size_t* host_sizes,
                                   void* stream) {
+  return scn_jpeg_encode_u8_opts(host_src_ptrs, n, width, height, channels, quality, nullptr, alloc_out, alloc_ctx,
+                                 host_sizes, stream);
+}
+
+extern "C" int scn_jpeg_encode_u8_opts(const uint8_t* const* host_src_ptrs, int n, int width, int height,
+                                       int channels, int quality, const scn_jpeg_options* opts, scn_alloc_fn alloc_out,
+                                       void* alloc_ctx, size_t* host_sizes, void* stream) {
   using namespace scn;
-  if (n < 0 || width <= 0 || height <= 0 || quality < 1 || quality > 100) return SCN_E_BADARG;
+  Settings set;
+  if (n < 0 || width <= 0 || height <= 0 || !settings(channels, quality, opts, &set)) return SCN_E_BADARG;
   if (channels != 1 && channels != 3) return SCN_E_UNSUPPORTED;
   if (width > kMaxDim || height > kMaxDim) return SCN_E_UNSUPPORTED;
   if (n == 0) return 0;
@@ -498,11 +802,12 @@ extern "C" int scn_jpeg_encode_u8(const uint8_t* const* host_src_ptrs, int n, in
   cudaStream_t st = (cudaStream_t)stream;
   cudaMemPool_t pool = scratch_pool();
   if (!pool) return (int)cudaErrorMemoryAllocation;
-  const Geom g = make_geom(width, height, channels);
+  const Geom g = make_geom(width, height, channels, set.hv);
   const uint32_t nm = g.mcus();
-  const Tables tables = make_tables(quality);
+  const Tables tables = make_tables(set.quality);
   Affixes ax;
-  if (!make_affixes(&ax, make_header(width, height, channels, quality), {}, {0xFF, 0xD9})) return SCN_E_UNSUPPORTED;
+  if (!make_affixes(&ax, make_header(width, height, channels, set.quality, set.hv), {}, {0xFF, 0xD9}))
+    return SCN_E_UNSUPPORTED;
 
   Scratch s{st, {}};
   int16_t* dcs = s.get<int16_t>((size_t)n * nm * g.bpm, pool);
@@ -512,21 +817,60 @@ extern "C" int scn_jpeg_encode_u8(const uint8_t* const* host_src_ptrs, int n, in
   if (!dcs || !acbits || !mcu_bit || !bits) return (int)cudaErrorMemoryAllocation;
   const dim3 mcu_grid((nm + kThreads - 1) / kThreads);
 
-  // DCs and AC bit counts, then per-frame scans into bit offsets
+  // optimised tables: per-frame AC counts, codes and headers in scratch
+  const bool optimize = opts && opts->optimize;
+  FrameTables ft = {nullptr, nullptr};
+  FramePrefixes fp = {nullptr, nullptr};
+  HeaderParts hp = {};
+  if (optimize) {
+    uint32_t* ac_hist = s.get<uint32_t>((size_t)n * 2 * 256, pool);
+    uint32_t* codes = s.get<uint32_t>((size_t)n * kCodeWords, pool);
+    uint8_t* prefix = s.get<uint8_t>((size_t)n * kMaxPrefix, pool);
+    uint32_t* prefix_len = s.get<uint32_t>((size_t)n, pool);
+    if (!ac_hist || !codes || !prefix || !prefix_len) return (int)cudaErrorMemoryAllocation;
+    const int rc = (int)cudaMemsetAsync(ac_hist, 0, (size_t)n * 2 * 256 * 4, st);
+    if (rc) return rc;
+    ft = {codes, ac_hist};
+    fp = {prefix, prefix_len};
+    // the Annex K header's parts around its DHT segments
+    const std::vector<uint8_t> full = make_header(width, height, channels, set.quality, set.hv);
+    size_t at = 2, dht = 0, sos = 0;
+    while (at + 4 <= full.size()) {
+      if (full[at + 1] == 0xC4 && !dht) dht = at;
+      if (full[at + 1] == 0xDA) sos = at;
+      at += 2 + ((size_t)full[at + 2] << 8 | full[at + 3]);
+    }
+    std::copy(full.begin(), full.begin() + dht, hp.head);
+    std::copy(full.begin() + sos, full.end(), hp.sos);
+    hp.head_len = (int)dht, hp.sos_len = (int)(full.size() - sos), hp.ntab = channels == 3 ? 2 : 1;
+  }
+
+  // DCs and AC bit counts, then per-frame scans into bit offsets; with optimised tables, first the symbol counts and
+  // the tables built from them
   auto measure = [&] {
     return for_each_chunk(n, [&](int i0, int cnt) {
       const PtrBatch src = gather<PtrBatch>(host_src_ptrs, i0, cnt);
       const MeasureOut mo = {dcs, acbits};
       const dim3 grid(mcu_grid.x, (unsigned)cnt);
-      const int e = launch_kernel("jpeg_mcu_kernel<measure>", st, [&] {
-        if (channels == 3)
-          jpeg_mcu_kernel<3, false><<<grid, kThreads, 0, st>>>(src, i0, g, tables, mo, EmitIn{});
-        else
-          jpeg_mcu_kernel<1, false><<<grid, kThreads, 0, st>>>(src, i0, g, tables, mo, EmitIn{});
+      int e = 0;
+      if (optimize) {
+        e = launch_kernel("jpeg_mcu_kernel<stats>", st, [&] {
+          launch_mcu<kStats>(channels, set.hv, grid, st, src, i0, g, tables, mo, EmitIn{}, FrameTables{nullptr,
+                                                                                                         ft.ac_hist});
+        });
+        if (!e)
+          e = launch_kernel("jpeg_table_kernel", st, [&] {
+            jpeg_table_kernel<<<cnt, 64, 0, st>>>(i0, nm, g.bpm, g.ny, dcs, ft.ac_hist, const_cast<uint32_t*>(ft.codes),
+                                                  const_cast<uint8_t*>(fp.bytes), const_cast<uint32_t*>(fp.len), hp);
+          });
+        if (e) return e;
+      }
+      e = launch_kernel("jpeg_mcu_kernel<measure>", st, [&] {
+        launch_mcu<kMeasure>(channels, set.hv, grid, st, src, i0, g, tables, mo, EmitIn{}, ft);
       });
       if (e) return e;
       return launch_kernel("jpeg_scan_kernel", st, [&] {
-        jpeg_scan_kernel<<<cnt, 1024, 0, st>>>(i0, nm, g.bpm, tables, dcs, acbits, mcu_bit, bits);
+        jpeg_scan_kernel<<<cnt, 1024, 0, st>>>(i0, nm, g.bpm, g.ny, tables, ft.codes, dcs, acbits, mcu_bit, bits);
       });
     });
   };
@@ -537,12 +881,31 @@ extern "C" int scn_jpeg_encode_u8(const uint8_t* const* host_src_ptrs, int n, in
     for (int j = 0; j < cnt; ++j) ei.stream_off[j] = stream_off[j];
     const dim3 grid(mcu_grid.x, (unsigned)cnt);
     return launch_kernel("jpeg_mcu_kernel<emit>", st, [&] {
-      if (channels == 3)
-        jpeg_mcu_kernel<3, true><<<grid, kThreads, 0, st>>>(src, i0, g, tables, MeasureOut{}, ei);
-      else
-        jpeg_mcu_kernel<1, true><<<grid, kThreads, 0, st>>>(src, i0, g, tables, MeasureOut{}, ei);
+      launch_mcu<kEmit>(channels, set.hv, grid, st, src, i0, g, tables, MeasureOut{}, ei, ft);
     });
   };
   return run_output_stage<FfStuffing>(n, st, pool, s, bits, nullptr, ax, measure, emit, alloc_out, alloc_ctx,
-                                      host_sizes);
+                                      host_sizes, fp);
+}
+
+extern "C" int scn_jpeg_optimal_table(const uint64_t* host_freq, uint8_t* host_bits, uint8_t* host_vals) {
+  using namespace scn;
+  if (!host_freq || !host_bits || !host_vals) return SCN_E_BADARG;
+  uint64_t* d_freq = nullptr;
+  uint8_t* d_out = nullptr;
+  int rc = (int)cudaMalloc(&d_freq, 256 * 8);
+  if (!rc) rc = (int)cudaMalloc(&d_out, 16 + 256 + 4);
+  if (!rc) rc = (int)cudaMemcpy(d_freq, host_freq, 256 * 8, cudaMemcpyHostToDevice);
+  if (!rc)
+    rc = launch_kernel("jpeg_gen_table_kernel", nullptr, [&] {
+      jpeg_gen_table_kernel<<<1, 32>>>(d_freq, d_out, d_out + 16, reinterpret_cast<int*>(d_out + 272));
+    });
+  uint8_t out[16 + 256 + 4];
+  if (!rc) rc = (int)cudaMemcpy(out, d_out, sizeof(out), cudaMemcpyDeviceToHost);
+  cudaFree(d_freq);
+  cudaFree(d_out);
+  if (rc) return rc;
+  std::copy(out, out + 16, host_bits);
+  std::copy(out + 16, out + 272, host_vals);
+  return 0;
 }

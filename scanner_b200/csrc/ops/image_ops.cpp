@@ -6,7 +6,8 @@
 //                 heuristic -- the file bytes differ, the decoded pixels are identical (lossless).
 //                 The GPU kernel of the op also writes JPEG (format "jpg"): scannertools encoded with
 //                 cv::imencode, and scn_jpeg_encode_u8 gives cv2.imencode's bytes exactly (HWC u8 frames with
-//                 1 or 3 channels, ImageEncoderArgs.quality, 95 when 0).  "png" on the GPU kernel copies the
+//                 1 or 3 channels, ImageEncoderArgs.quality, 95 when 0; cv2's sampling, optimize and luma /
+//                 chroma quality options through scn_jpeg_encode_u8_opts).  "png" on the GPU kernel copies the
 //                 frames to the host and writes the same PNG as the CPU kernel.
 //   ImageDecoder  PNG bytes -> frame (the op pipelines pair with it: examples/tutorials/
 //                 05_sources_sinks.py:41-47; upstream it lives in scannertools and calls
@@ -215,6 +216,12 @@ class ImageEncoderKernel : public BatchedKernel {
       RESULT_ERROR(&valid_, "Invalid format type specified to ImageEncoder: %s. Valid types are: png.", fmt.c_str());
       return;
     }
+    if (!args.sampling().empty() || args.optimize() || args.luma_quality() || args.chroma_quality()) {
+      RESULT_ERROR(&valid_, "ImageEncoder sampling, optimize, luma_quality and chroma_quality are JPEG options; "
+                   "format is %s",
+                   fmt.c_str());
+      return;
+    }
     valid_.set_success(true);
   }
   void validate(Result* result) override { result->CopyFrom(valid_); }
@@ -265,6 +272,33 @@ class ImageEncoderKernelGPU : public BatchedKernel {
       RESULT_ERROR(&valid_, "ImageEncoder quality %d is outside [1, 100]", quality_);
       return;
     }
+    const std::string& sampling = args.sampling();
+    const bool options = !sampling.empty() || args.optimize() || args.luma_quality() || args.chroma_quality();
+    if (options && !jpeg_) {
+      RESULT_ERROR(&valid_, "ImageEncoder sampling, optimize, luma_quality and chroma_quality are JPEG options; "
+                   "format is %s",
+                   fmt.c_str());
+      return;
+    }
+    if (!sampling.empty()) {
+      static const struct { const char* name; int hv; } kModes[] = {
+          {"444", SCN_JPEG_444}, {"422", SCN_JPEG_422}, {"420", SCN_JPEG_420}, {"440", SCN_JPEG_440},
+          {"411", SCN_JPEG_411}};
+      for (const auto& m : kModes)
+        if (sampling == m.name) opts_.sampling = m.hv;
+      if (!opts_.sampling) {
+        RESULT_ERROR(&valid_, "ImageEncoder sampling %s is not one of 444, 422, 420, 440, 411", sampling.c_str());
+        return;
+      }
+    }
+    for (int q : {args.luma_quality(), args.chroma_quality()})
+      if (q < 0 || q > 100) {
+        RESULT_ERROR(&valid_, "ImageEncoder luma / chroma quality %d is outside [1, 100]", q);
+        return;
+      }
+    opts_.luma_quality = args.luma_quality();
+    opts_.chroma_quality = args.chroma_quality();
+    opts_.optimize = args.optimize() ? 1 : 0;
     valid_.set_success(true);
   }
   void validate(Result* result) override { result->CopyFrom(valid_); }
@@ -344,9 +378,9 @@ class ImageEncoderKernelGPU : public BatchedKernel {
     std::vector<size_t> sizes(n);
     staging_ = nullptr;
     cudaStream_t stream = (cudaStream_t)device_stream(device_);
-    const int rc = scn_jpeg_encode_u8(src.data(), (int)n, f0->width(), f0->height(), f0->channels(), quality_,
-                                      &ImageEncoderKernelGPU::alloc_on, this, sizes.data(), stream);
-    if (rc != 0) LOG(FATAL) << "scn_jpeg_encode_u8 failed with code " << rc;
+    const int rc = scn_jpeg_encode_u8_opts(src.data(), (int)n, f0->width(), f0->height(), f0->channels(), quality_,
+                                           &opts_, &ImageEncoderKernelGPU::alloc_on, this, sizes.data(), stream);
+    if (rc != 0) LOG(FATAL) << "scn_jpeg_encode_u8_opts failed with code " << rc;
     // one copy of the packed files to the host, in the synchronisation the encoder needs anyway
     u8* block = new_block_buffer_sizes(CPU_DEVICE, sizes);
     size_t total = 0;
@@ -366,6 +400,7 @@ class ImageEncoderKernelGPU : public BatchedKernel {
   DeviceHandle device_;
   bool jpeg_ = false;
   int quality_ = 95;
+  scn_jpeg_options opts_ = {0, 0, 0, 0};  // sampling, luma and chroma quality, optimize: 0 when absent
   u8* staging_ = nullptr;  // the device buffer scn_jpeg_encode_u8 writes the files of one run into
   Result valid_;
 };

@@ -281,24 +281,41 @@ def convert_color(frames, code, width=None, height=None):
     return _per_shape(frames, run)
 
 
-def jpeg_encode_bound(width, height, channels=3):
-    """Bytes no JPEG file of that geometry exceeds at any quality (scn_jpeg_encode_bound)."""
-    return cabi.lib().scn_jpeg_encode_bound(width, height, channels)
+# ImageEncoder's `sampling` names -> the luma sampling factors h << 4 | v of scn_jpeg_options
+JPEG_SAMPLING = {"444": 0x11, "422": 0x21, "420": 0x22, "440": 0x12, "411": 0x41}
 
 
-def jpeg_encode(frames, quality=95):
+def _jpeg_options(sampling, luma_quality, chroma_quality, optimize=False):
+    """-> scn_jpeg_options; an unknown sampling name becomes a code the library refuses (SCN_E_BADARG)"""
+    code = 0 if sampling is None else JPEG_SAMPLING.get(sampling, -1)
+    return cabi.JpegOptions(code, int(luma_quality or 0), int(chroma_quality or 0), int(optimize))
+
+
+def jpeg_encode_bound(width, height, channels=3, *, sampling=None, luma_quality=0, chroma_quality=0,
+                      optimize=False):
+    """Bytes no JPEG file of that geometry and those options exceeds at any quality (scn_jpeg_encode_bound_opts);
+    0 if they are refused."""
+    o = _jpeg_options(sampling, luma_quality, chroma_quality, optimize)
+    return cabi.lib().scn_jpeg_encode_bound_opts(width, height, channels, ctypes.byref(o))
+
+
+def jpeg_encode(frames, quality=95, *, sampling=None, luma_quality=0, chroma_quality=0, optimize=False):
     """Baseline JPEG files of uint8 frames, byte for byte cv2.imencode('.jpg', bgr, [cv2.IMWRITE_JPEG_QUALITY,
     quality]) with bgr the frame's channels reversed (frames are RGB) or the gray frame itself.
+    With options, cv2's IMWRITE_JPEG_SAMPLING_FACTOR ("444", "422", "420" (the default), "440" or "411"),
+    IMWRITE_JPEG_LUMA_QUALITY and IMWRITE_JPEG_CHROMA_QUALITY (1-100, 0 for absent) under cv2's rules, and
+    IMWRITE_JPEG_OPTIMIZE (Huffman tables built per frame) (include/scn_kernels.h, scn_jpeg_encode_u8_opts).
 
     frames: (N,H,W,C) uint8 CUDA tensor or a list of (H,W,C) tensors, shapes may differ (one call per run of
     equal shape); C is 3 or 1, and a frame need not be aligned.  -> list of N bytes objects.  Synchronises
     the current stream."""
     L = cabi.lib()
+    opts = _jpeg_options(sampling, luma_quality, chroma_quality, optimize)
 
     def run(src_ptrs, h, w, c, device):
         sp, k1 = cabi.ptr_array(src_ptrs)
-        return _encode("scn_jpeg_encode_u8", len(src_ptrs), device, lambda cb, sizes: L.scn_jpeg_encode_u8(
-            sp, len(src_ptrs), w, h, c, int(quality), cb, None, sizes, _stream()))
+        return _encode("scn_jpeg_encode_u8", len(src_ptrs), device, lambda cb, sizes: L.scn_jpeg_encode_u8_opts(
+            sp, len(src_ptrs), w, h, c, int(quality), ctypes.byref(opts), cb, None, sizes, _stream()))
 
     if isinstance(frames, torch.Tensor):
         _need_cuda(frames)
