@@ -144,6 +144,40 @@ SCN_API int scn_box_blur_u8c3_strided(const uint8_t* src, size_t stride_bytes, i
                               int height, int kernel_size, uint8_t* dst, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * GaussianBlur  (cv::GaussianBlur(frame, out, Size(kw, kh), sigma_x, sigma_y, border) on CV_8U frames).
+ * Bit-exact vs cv2.GaussianBlur, whose 8-bit path is fixed point: taps with 8 fraction bits summing to 256, a
+ * horizontal pass into 8.8 row sums and a vertical pass rounded as (s + 2^15) >> 16.
+ *
+ * scn_gaussian_blur_border_code: cv2's number of a border name: "", "BORDER_DEFAULT", "BORDER_REFLECT_101" (and
+ *   "BORDER_REFLECT101") -> 4, "BORDER_REPLICATE" -> 1, "BORDER_REFLECT" -> 2.  SCN_E_UNSUPPORTED for cv2's other
+ *   borders (BORDER_CONSTANT, _WRAP, _TRANSPARENT, _ISOLATED), SCN_E_BADARG for any other name.
+ * scn_gaussian_blur_borders: the supported names, for error messages.
+ * scn_gaussian_blur_plan_bytes / _plan_fill: the plan of one argument set, built on the host: both axes' taps as
+ *   cv2 builds them (ksize 0 from sigma as cvRound(sigma * 6 + 1) | 1; sigma <= 0 from ksize; sigma_y <= 0 means
+ *   sigma_x).  SCN_E_BADARG for an even or negative ksize, ksize 0 with sigma <= 0, a non-finite sigma, a border
+ *   code other than 1, 2, 4 or a null plan; SCN_E_UNSUPPORTED for a ksize (given or derived) above 31.  The plan is
+ *   a host buffer: its taps travel to the kernels in the launch's parameter block, so nothing is copied to the
+ *   device and the plan may be freed when the launch call returns.
+ * scn_gaussian_blur_u8: n dense HxWxC frames (C = 1 or 3), any base alignment, pointer list -> n dense frames of the
+ *   same shape; batches over 64 frames are split into launches.
+ * scn_gaussian_blur_nv12: n NV12 surfaces as scn_nv12_to_rgb24 takes them -> n dense HxWx3 frames, identical to
+ *   scn_nv12_to_rgb24 followed by scn_gaussian_blur_u8; the RGB24 frame is never written.
+ * Refused before any launch: a null or malformed plan (SCN_E_PLAN); n or a side below 0, C not 1 or 3, null
+ * pointer lists with n > 0, a frame of more than INT_MAX pixels, or for NV12 an odd or zero side or a pitch below
+ * the width (SCN_E_BADARG); a row of more than INT_MAX bytes or more than 1,048,560 rows (SCN_E_UNSUPPORTED).
+ */
+SCN_API int scn_gaussian_blur_border_code(const char* name);
+SCN_API const char* scn_gaussian_blur_borders(void);
+SCN_API size_t scn_gaussian_blur_plan_bytes(void);
+SCN_API int scn_gaussian_blur_plan_fill(int kernel_width, int kernel_height, double sigma_x, double sigma_y,
+                                        int border, void* host_plan);
+SCN_API int scn_gaussian_blur_u8(const void* plan, const uint8_t* const* host_src_ptrs, int n, int width, int height,
+                                 int channels, uint8_t* const* host_dst_ptrs, void* stream);
+SCN_API int scn_gaussian_blur_nv12(const void* plan, const uint8_t* const* host_luma_ptrs,
+                                   const uint8_t* const* host_chroma_ptrs, size_t pitch, int n, int width, int height,
+                                   uint8_t* const* host_dst_ptrs, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * NV12 -> RGB24  (replaces convertNV12toRGBA, scanner/util/image.cu:229-239 and its kernel
  *                 :109-200; called from NVIDIAVideoDecoder::get_frame,
  *                 scanner/video/nvidia/nvidia_video_decoder.cpp:288-296)

@@ -59,6 +59,12 @@ SIGNATURES = {
     "scn_nv12_hist_resize": (_c.c_int, [_PP, _PP, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _VP, _PP,
                                         _c.c_int, _c.c_int, _VP, _VP]),
     "scn_frame_digest": (_c.c_int, [_PP, _c.c_int, _c.c_size_t, _VP, _VP]),
+    "scn_gaussian_blur_border_code": (_c.c_int, [_c.c_char_p]),
+    "scn_gaussian_blur_borders": (_c.c_char_p, []),
+    "scn_gaussian_blur_plan_bytes": (_c.c_size_t, []),
+    "scn_gaussian_blur_plan_fill": (_c.c_int, [_c.c_int, _c.c_int, _c.c_double, _c.c_double, _c.c_int, _VP]),
+    "scn_gaussian_blur_u8": (_c.c_int, [_VP, _PP, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _PP, _VP]),
+    "scn_gaussian_blur_nv12": (_c.c_int, [_VP, _PP, _PP, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _PP, _VP]),
     "scn_convert_color_code": (_c.c_int, [_c.c_char_p]),
     "scn_convert_color_name": (_c.c_char_p, [_c.c_int]),
     "scn_convert_color_channels": (_c.c_int, [_c.c_int, _c.POINTER(_c.c_int), _c.POINTER(_c.c_int)]),

@@ -900,6 +900,7 @@ class Client:
             self._op_protos["Blur"] = {"init": std["BlurArgs"]}
             self._op_protos["Resize"] = {"stream": std["ResizeArgs"]}
             self._op_protos["ConvertColor"] = {"stream": std["ConvertColorArgs"]}
+            self._op_protos["GaussianBlur"] = {"init": std["GaussianBlurArgs"]}
             self._op_protos["ImageEncoder"] = {"init": std["ImageEncoderArgs"]}
             self._op_protos["OpticalFlowTVL1"] = {"init": std["OpticalFlowTVL1Args"]}
 

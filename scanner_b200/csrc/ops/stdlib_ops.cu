@@ -367,6 +367,98 @@ REGISTER_OP(Blur).frame_input("frame").frame_output("frame").protobuf_name("Blur
 REGISTER_KERNEL(Blur, BlurKernelGPU).device(DeviceType::GPU).batch(16).num_devices(1);
 
 // ---------------------------------------------------------------------------------------------
+// GaussianBlur: cv2.GaussianBlur(frame, (kernel_width, kernel_height), sigma_x, sigma_y, border), bit-exact, on
+// HxWx3 and HxWx1 uint8 frames and on decoded NV12 elements (blurred from the RGB24 frame the decoder would have
+// delivered, without writing it).  Arguments the kernels refuse fail the run at the first batch, with the row.
+class GaussianBlurKernelGPU : public BatchedKernel {
+ public:
+  GaussianBlurKernelGPU(const KernelConfig& config) : BatchedKernel(config), device_(config.devices[0]) {
+    GaussianBlurArgs a;
+    if (!a.ParseFromArray(config.args.data(), (int)config.args.size())) {
+      args_problem_ = "could not parse GaussianBlurArgs";
+      return;
+    }
+    const int border = scn_gaussian_blur_border_code(a.border().c_str());
+    if (border < 0) {
+      args_problem_ = std::string(border == SCN_E_UNSUPPORTED ? "unsupported" : "unknown") + " border '" +
+                      a.border() + "'; supported: " + scn_gaussian_blur_borders();
+      return;
+    }
+    plan_.resize(scn_gaussian_blur_plan_bytes());
+    const int rc = scn_gaussian_blur_plan_fill(a.kernel_width(), a.kernel_height(), a.sigma_x(), a.sigma_y(), border,
+                                               plan_.data());
+    if (rc != 0)
+      args_problem_ = std::string(rc == SCN_E_UNSUPPORTED ? "unsupported" : "bad") + " ksize " +
+                      std::to_string(a.kernel_width()) + "x" + std::to_string(a.kernel_height()) + " with sigma " +
+                      std::to_string(a.sigma_x()) + ", " + std::to_string(a.sigma_y()) +
+                      " (ksize is odd, 1-31 per axis, or 0 with sigma > 0 and a derived size of at most 31)";
+  }
+
+  void execute(const BatchedElements& input_columns, BatchedElements& output_columns) override {
+    const Elements& frames = input_columns[0];
+    if (frames.empty()) return;
+    CU_CHECK(cudaSetDevice(device_.id));
+    for_each_run(frames, [&](size_t i0, size_t i1, const Frame* f0) {
+      const i32 n = (i32)(i1 - i0);
+      const bool nv12 = is_nv12(f0);
+      const int w = pic_width(f0), h = pic_height(f0), c = nv12 ? 3 : f0->channels();
+      std::string why = args_problem_;
+      if (why.empty() && nv12)
+        why = rgb8_problem(f0);
+      else if (why.empty() && ((proto::FrameType)f0->type != proto::U8 || (c != 1 && c != 3)))
+        why = "expects HxWx3 or HxWx1 uint8 frames, got " + std::to_string(f0->height()) + "x" +
+              std::to_string(f0->width()) + "x" + std::to_string(c) + " type " +
+              std::to_string((int)(proto::FrameType)f0->type);
+      if (why.empty()) {
+        std::vector<Frame*> outs = new_frames(device_, FrameInfo(h, w, c, FrameType::U8), n);
+        std::vector<const u8*> src;
+        std::vector<u8*> dst;
+        for (i32 i = 0; i < n; ++i) {
+          src.push_back(frames[i0 + i].as_const_frame()->data);
+          dst.push_back(outs[i]->data);
+        }
+        int rc;
+        if (nv12) {
+          std::vector<const u8*> chroma;
+          for (const u8* p : src) chroma.push_back(p + (size_t)w * h);
+          rc = scn_gaussian_blur_nv12(plan_.data(), src.data(), chroma.data(), (size_t)w, n, w, h, dst.data(),
+                                      device_stream(device_));
+        } else {
+          rc = scn_gaussian_blur_u8(plan_.data(), src.data(), n, w, h, c, dst.data(), device_stream(device_));
+        }
+        if (rc == 0) {
+          for (i32 i = 0; i < n; ++i) insert_frame(output_columns[0], outs[i]);
+          return;
+        }
+        for (Frame* f : outs) {
+          delete_buffer(device_, f->data);
+          delete f;
+        }
+        why = std::string(nv12 ? "scn_gaussian_blur_nv12" : "scn_gaussian_blur_u8") + " failed with code " +
+              std::to_string(rc) + " on " + std::to_string(n) + " " + std::to_string(h) + "x" + std::to_string(w) +
+              " frames";
+      }
+      report_kernel_error("GaussianBlur, row " + std::to_string(frames[i0].index) + ": " + why);
+      for (i32 i = 0; i < n; ++i) output_columns[0].push_back(Element());
+    });
+  }
+
+ private:
+  DeviceHandle device_;
+  // the host plan of the op's one argument set: built once, its taps travel in each launch's parameter block
+  std::vector<u8> plan_;
+  std::string args_problem_;  // why the arguments are refused; empty when they are not
+};
+
+REGISTER_OP(GaussianBlur).frame_input("frame").frame_output("frame").protobuf_name("GaussianBlurArgs");
+
+REGISTER_KERNEL(GaussianBlur, GaussianBlurKernelGPU)
+    .device(DeviceType::GPU)
+    .batch(64)
+    .num_devices(1)
+    .input_layout("frame", FrameLayout::NV12);
+
+// ---------------------------------------------------------------------------------------------
 // OpticalFlow: stencil {0,1}, Farneback with the reference's constructor arguments
 // (tests/test_ops.cpp:68-69), output Frame(H, W, 2, F32) on the GPU (:85-87).
 class OpticalFlowKernelGPU : public StenciledKernel, public VideoKernel {

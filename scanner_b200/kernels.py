@@ -281,6 +281,64 @@ def convert_color(frames, code, width=None, height=None):
     return _per_shape(frames, run)
 
 
+def gaussian_blur_plan(ksize, sigma_x, sigma_y=0.0, border=""):
+    """The host plan (a numpy byte array) of cv2.GaussianBlur's arguments.  ksize is (width, height) or one int for
+    both; border is a cv2 border name.  Raises for refused arguments, with what is supported."""
+    L = cabi.lib()
+    kw, kh = (ksize, ksize) if isinstance(ksize, int) else ksize
+    code = L.scn_gaussian_blur_border_code(str(border).encode())
+    if code < 0:
+        kind = "not supported" if code == -2 else "unknown"
+        raise cabi.ScnError(f"GaussianBlur border {border!r} is {kind}; supported: "
+                            f"{L.scn_gaussian_blur_borders().decode()}")
+    plan = np.zeros(L.scn_gaussian_blur_plan_bytes(), np.uint8)
+    cabi.check(L.scn_gaussian_blur_plan_fill(int(kw), int(kh), float(sigma_x), float(sigma_y), code,
+                                             plan.ctypes.data), "scn_gaussian_blur_plan_fill")
+    return plan
+
+
+def gaussian_blur(frames, ksize, sigma_x, sigma_y=0.0, border=""):
+    """cv2.GaussianBlur(frame, ksize, sigma_x, sigmaY=sigma_y, borderType=border) on the GPU, bit-exact.
+
+    frames: (N,H,W,C) uint8 CUDA tensor, C = 1 or 3 -> the same shape; or a list of (H,W,C) tensors, shapes may
+    differ -> list (one launch per run of equal shape)."""
+    plan = gaussian_blur_plan(ksize, sigma_x, sigma_y, border)
+    L = cabi.lib()
+
+    def run(src_ptrs, h, w, c, device):
+        out = torch.empty((len(src_ptrs), h, w, c), dtype=torch.uint8, device=device)
+        sp, k1 = cabi.ptr_array(src_ptrs)
+        dp, k2 = cabi.ptr_array([out.data_ptr() + i * h * w * c for i in range(len(src_ptrs))])
+        cabi.check(L.scn_gaussian_blur_u8(plan.ctypes.data, sp, len(src_ptrs), w, h, c, dp, _stream()),
+                   "scn_gaussian_blur_u8")
+        return out
+
+    if isinstance(frames, torch.Tensor):
+        _need_cuda(frames)
+        assert frames.dtype == torch.uint8 and frames.dim() == 4
+        frames = frames.contiguous()
+        n, h, w, c = frames.shape
+        return run([frames.data_ptr() + i * h * w * c for i in range(n)], h, w, c, frames.device)
+    return _per_shape(frames, run)
+
+
+def nv12_gaussian_blur(surfaces, width, height, ksize, sigma_x, sigma_y=0.0, border=""):
+    """gaussian_blur of the RGB24 frames nv12_to_rgb would give for (N, H*3/2, pitch) NV12 surfaces ->
+    (N,H,W,3), without writing those frames."""
+    plan = gaussian_blur_plan(ksize, sigma_x, sigma_y, border)
+    _need_cuda(surfaces)
+    surfaces = surfaces.contiguous()
+    n = surfaces.shape[0]
+    lum, chr_, pitch = _surface_ptrs(surfaces, height)
+    out = torch.empty((n, height, width, 3), dtype=torch.uint8, device=surfaces.device)
+    lp, k1 = cabi.ptr_array(lum)
+    cp, k2 = cabi.ptr_array(chr_)
+    op, k3 = cabi.ptr_array([out.data_ptr() + i * height * width * 3 for i in range(n)])
+    cabi.check(cabi.lib().scn_gaussian_blur_nv12(plan.ctypes.data, lp, cp, pitch, n, width, height, op, _stream()),
+               "scn_gaussian_blur_nv12")
+    return out
+
+
 # ImageEncoder's `sampling` names -> the luma sampling factors h << 4 | v of scn_jpeg_options
 JPEG_SAMPLING = {"444": 0x11, "422": 0x21, "420": 0x22, "440": 0x12, "411": 0x41}
 
